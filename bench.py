@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- BPR triplet-updates/s and ranked-users/s on 1/2/4/8 B200 vs the reference CPU path.
+"""bench.py -- BPR triplet-updates/s and ranked-users/s on 1/2/4/8 H100 vs the reference CPU path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload c3|c2]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload c3|c2] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (default, BASELINE.json configs[2] -- the north_star target): ONE synthetic model of 10 M users x
@@ -11,7 +11,7 @@ for every N; `--gpus N` shards it by interaction count: rank r owns blocks [8 r 
 (STRONG scaling: total work fixed).  The 1 M-item matrix V (512 MB) and the biases are replicated and the
 item changes are exchanged once per epoch inside the timed region (one fused NVLink peer-memory kernel per tensor, or
 delta kernels + NCCL all-reduce with --exchange nccl; rule: mean over the ranks that changed a row).  N = 1 holds the
-whole model on one GPU (about 35 GB of the 180 GB).
+whole model on one GPU (about 35 GB of the 80 GB).
 
 A "step" is one BPR epoch over the whole model = 1 B sampled triplets in total (what one call of the
 reference's BPR._fit_sgd does, cornac/models/bpr/recom_bpr.pyx:208-269), i.e. nnz / N per rank.
@@ -22,8 +22,11 @@ e2e    = the same through the host-buffer entry the plug-in's fit() uses (engine
          pinned-host CSR + factors -> H2D -> prepare -> one epoch -> D2H, per rank on its shard;
 roofline / cpu_baseline / per_rank / rank (configs[4]: all 10 M users of the trained model ranked against
 the 1 M items, top-100) / mf (configs[3]: MF k = 128 on the same 10 M x 1 M x 1 B rating list) ride along.
---impl reference times the reference's own Cython/OpenMP kernel (baseline/_ref) on the host cores the
+--impl reference times the reference's own Cython/OpenMP kernel (oracle/_ref) on the host cores the
 process actually owns, on a bounded sample of the same workload.
+--dump-outputs DIR writes, after the timed steps, what the last timed epoch left to its caller: a fixed, seeded
+sample of rows of U and V, all of B and the (correct, skipped) counts, as DIR/<name>.npy (rank r > 0 adds _r<r>).
+The inputs depend only on the arguments, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -213,7 +216,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def tensor_peak():
@@ -224,7 +227,7 @@ def tensor_peak():
         for key in ("bf16_tflops_sustained", "bf16_tflops"):
             if key in d:
                 return float(d[key]), "measured sustained (MEASURED_PEAKS.json)"
-    return 1400.0, "fallback sustained (B200_PROFILING.md)"
+    return 989.0, "fallback (H100 SXM data sheet, dense FP16; not reached in practice)"
 
 
 def algorithmic_bytes(k, updates, skipped, mean_deg):
@@ -282,12 +285,12 @@ def measured_traffic(workload, kernel_name, samples_per_launch):
 
 # --------------------------------------------------------------------------------------
 def ref_path():
-    return os.path.join(ROOT, "baseline", "_ref")
+    return os.path.join(ROOT, "oracle", "_ref")
 
 
 def reference_fit_sgd_runner(indptr, indices, n_items, k, lr, reg, n_threads):
     """Returns (run_epoch() -> (correct, skipped), kind, cores).  Uses the UNMODIFIED compiled
-    reference (baseline/_ref: cornac.models.bpr.recom_bpr.BPR._fit_sgd + RNGVector) when it is
+    reference (oracle/_ref: cornac.models.bpr.recom_bpr.BPR._fit_sgd + RNGVector) when it is
     importable, else the oracle's OpenMP port."""
     ref = ref_path()
     n_users = len(indptr) - 1
@@ -380,7 +383,10 @@ def main():
     ap.add_argument("--scale", type=float, default=1.0, help="shrink users and interactions (debug only; result then INVALID)")
     ap.add_argument("--workload", default="c3", choices=sorted(WORKLOADS),
                     help="c3 = BASELINE configs[2] (default, the north_star target); c2 = configs[1]")
-    ap.add_argument("--atomic", type=int, default=1, help="1: red.global.add scatter (default), 0: plain racy stores")
+    ap.add_argument("--atomic", type=int, default=1, help="Hogwild scatter: 1 red.global.add (default, what fit() uses), 0 plain racy stores")
+    ap.add_argument("--deterministic", type=int, default=1,
+                    help="1: the timed epochs run in deterministic rounds, so their outputs repeat run to run (default); the Hogwild "
+                         "kernels are then timed in a separate leg (`hogwild`); 0: the timed epochs are Hogwild epochs")
     ap.add_argument("--blocked", type=int, default=1, help="1: cache-blocked sample order (default, what fit() uses), 0: i.i.d. order")
     ap.add_argument("--exchange", default="auto", choices=["auto", "p2p", "nccl"],
                     help="item-replica exchange at N > 1: p2p = one fused NVLink kernel per tensor, nccl = delta kernels + all-reduce")
@@ -388,7 +394,11 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-rank", action="store_true")
     ap.add_argument("--no-mf", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (sampled U / V rows, B, counts) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        raise SystemExit("bench.py: --steps must be >= 1 and --warmup >= 0")
 
     # stdout carries exactly ONE line, the JSON record: everything else any library prints to fd 1 (NCCL's INFO log goes
     # to stdout by default) is sent to stderr, where the NCCL init lines ("... nranks N ...") stay visible.
@@ -449,7 +459,7 @@ def main():
 
     def epoch(e):
         engine.bpr_epoch(data, W["n_items"], U, V, B, W["lr"], W["reg"], W["use_bias"], key + rank, e, stats,
-                         atomic=bool(args.atomic), blocked=bool(args.blocked))
+                         atomic=bool(args.atomic), blocked=bool(args.blocked), deterministic=bool(args.deterministic))
 
     def barrier():
         if world > 1:
@@ -476,6 +486,8 @@ def main():
     ev0.record()
     for e in range(args.steps):
         a, b, c = step_ev[e]
+        if e == args.steps - 1:
+            stats_before_last = stats.clone()
         a.record()
         epoch(args.warmup + e)
         b.record()
@@ -486,6 +498,8 @@ def main():
     barrier()
     clocks.window_end()
     launches = int(L.b200_kernel_launches()) - launches0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, U, V, B, stats - stats_before_last, rank, world)
     clk = clocks.stop() if rank == 0 else None
     ms_total = ev0.elapsed_time(ev1)
     kern_list = [a.elapsed_time(b) for a, b, _ in step_ev]
@@ -507,8 +521,9 @@ def main():
     # ---- roofline of the dominant kernel, per rank (every rank launches the same kernel on nnz / N samples)
     peak, peak_src = measured_peaks()
     g_lanes = min(32, max(4, k // 4))
-    kernel_name = ("bpr_hogwild_stream_kernel<G=%d,%s,D=2>" if (k % 4 == 0 and g_lanes >= 32) else "bpr_hogwild_chunk_kernel<G=%d,NPL=1,VEC,%s>") \
+    hog_name = ("bpr_hogwild_stream_kernel<G=%d,%s,D=2>" if (k % 4 == 0 and g_lanes >= 32) else "bpr_hogwild_chunk_kernel<G=%d,NPL=1,VEC,%s>") \
         % (g_lanes, "ATOMIC" if args.atomic else "PLAIN")
+    kernel_name = "bpr_det_grad_kernel + bpr_det_apply_kernel" if args.deterministic else hog_name
     fracs = []
     for r in range(world):
         upd_r, skp_r = allr[r, 1] / args.steps, allr[r, 2] / args.steps
@@ -545,6 +560,33 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
+    # ---- the Hogwild kernels (what fit() runs) on the same model, continuing from the timed epochs: their results differ
+    #      from run to run (samples read rows while others update them), so they are timed here but not dumped
+    hogwild = None
+    if args.deterministic:
+        hev = [(ev(), ev()) for _ in range(args.steps)]
+        stats.zero_()
+        barrier()
+        for e in range(args.steps):
+            hev[e][0].record()
+            engine.bpr_epoch(data, W["n_items"], U, V, B, W["lr"], W["reg"], W["use_bias"], key + rank, 1000 + e, stats,
+                             atomic=bool(args.atomic), blocked=bool(args.blocked))
+            hev[e][1].record()
+        barrier()
+        h_ms = over_ranks(float(np.mean([a.elapsed_time(b) for a, b in hev])))
+        h_skipped = float(stats[1].item())
+        h_upd = nnz * args.steps - h_skipped
+        if world > 1:
+            t = torch.tensor([h_upd], device=dev, dtype=torch.float64)
+            dist.all_reduce(t)
+            h_upd = float(t.item())
+        h_gbs = algorithmic_bytes(k, h_upd / args.steps / world, h_skipped / args.steps, mean_deg) / (h_ms * 1e-3) / 1e9
+        hogwild = {"value": round(h_upd / args.steps / (h_ms * 1e-3), 1), "unit": "updates/s", "ms_per_step": round(h_ms, 3),
+                   "steps": args.steps, "kernel": hog_name,
+                   "roofline": {"bound": "hbm", "achieved": round(h_gbs, 1), "peak": peak, "unit": "GB/s", "frac": round(h_gbs / peak, 4)},
+                   "note": "Hogwild epochs (the kernels fit() runs) on the same model, after the timed epochs; max over ranks, "
+                           "no item exchange; results differ from run to run, so they are not dumped"}
+
     # the pair store / membership table are only needed by the epochs
     data.pairs = data.table = None
     if sync is not None and hasattr(sync, "failed") and sync.failed():
@@ -569,7 +611,7 @@ def main():
     # ---- configs[3]: MF on the same rating list, all ranks
     mf_metric = None
     if not args.no_mf:
-        mf_metric = run_mf(W, engine, data, dev, world, over_ranks, exchange=args.exchange)
+        mf_metric = run_mf(W, engine, data, dev, world, over_ranks, exchange=args.exchange, steps=args.steps)
 
     # ---- CPU baseline on rank 0, N = 1 only
     cpu_baseline = None
@@ -590,10 +632,11 @@ def main():
             "config": {"workload": workload_text(W, world),
                        "step": "one epoch over the whole model = %d sampled triplets (%d per rank; Hogwild, on-device Philox sampling)"
                                % (W["nnz"], nnz),
-                       "l2": "working set per rank (U %d MB + V %d MB + pair store %d MB + membership table) exceeds the 126 MB L2; no flush needed"
+                       "l2": "working set per rank (U %d MB + V %d MB + pair store %d MB + membership table) exceeds the 50 MB L2; no flush needed"
                              % (n_local * k * 4 // 1000000, W["n_items"] * k * 4 // 1000000, nnz * 8 // 1000000),
                        "parallelism": "users sharded x%d by interaction count, items replicated, 1 exchange of item changes per epoch (mean over the ranks that changed a row)" % world,
-                       "scatter": "red.global.add.v4.f32" if args.atomic else "st.global.cg.v4.f32 (Hogwild)",
+                       "scatter": ("deterministic rounds of <= 16384 samples, updates summed in 2^-40 fixed point" if args.deterministic
+                                   else "red.global.add.v4.f32 (Hogwild)" if args.atomic else "st.global.cg.v4.f32 (Hogwild)"),
                        "sample_order": ("cache-blocked: %d windows of the interaction list x %d item blocks per rank (b200_bpr_block_plan); "
                                         "same per-epoch law as the i.i.d. order" % engine.bpr_block_plan(n_local, W["n_items"], k))
                                        if args.blocked else "i.i.d. (Philox counter order)"},
@@ -603,7 +646,7 @@ def main():
             "gpu_launches": int(allr[:, 5].sum()),
             "gpu_launches_note": "b200_kernel_launches() delta over the timed region, summed over ranks (NCCL's own kernels not counted)",
             "clocks": clk, "roofline": roofline, "per_rank": per_rank, "cpu_baseline": cpu_baseline, "e2e": e2e,
-            "rank": rank_metric, "mf": mf_metric, "host": host_cores(),
+            "hogwild": hogwild, "rank": rank_metric, "mf": mf_metric, "host": host_cores(),
         }
         if args.scale != 1.0:
             out["INVALID"] = "scaled-down debug run (--scale %g)" % args.scale
@@ -613,6 +656,31 @@ def main():
         dist.barrier()
         dist.destroy_process_group()
     return 0
+
+
+DUMP_ROWS = 32768                                   # sampled rows of U (over all ranks) and of V: 2 x 16 MB at k = 128
+
+
+def dump_outputs(out_dir, U, V, B, last_stats, rank, world):
+    """The arrays the timed BPR epochs leave to their caller, after the last timed step: a fixed sample of U's rows
+    (seeded, independent of the build; DUMP_ROWS / world per rank), and on rank 0 only a fixed sample of V's rows and all
+    of B (replicated on every rank), plus the (correct, skipped) counts of the last timed step, as float32 / float64 .npy."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = "" if rank == 0 else "_r%d" % rank
+    rng = np.random.RandomState(2024)
+    u_rows = np.sort(rng.choice(U.shape[0], min(DUMP_ROWS // world, U.shape[0]), replace=False))
+    v_rows = np.sort(rng.choice(V.shape[0], min(DUMP_ROWS, V.shape[0]), replace=False))
+    pick = lambda T, rows: T.index_select(0, torch.from_numpy(rows).to(T.device)).cpu().numpy().astype(np.float32)
+    arrays = {"U_sample": pick(U, u_rows), "U_sample_rows": u_rows.astype(np.float64),
+              "stats": last_stats.cpu().numpy().astype(np.float64)}
+    if rank == 0:
+        arrays.update({"V_sample": pick(V, v_rows), "V_sample_rows": v_rows.astype(np.float64),
+                       "B": B.cpu().numpy().astype(np.float32)})
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + sfx + ".npy"), a)
+    log("[bench] wrote %s to %s" % (", ".join(sorted(arrays)), out_dir))
 
 
 def run_e2e(args, W, engine, indptr, indices, blocks, dev, world, rank):
@@ -628,7 +696,7 @@ def run_e2e(args, W, engine, indptr, indices, blocks, dev, world, rank):
     nnz = h_indices.numel()
     h2d = sum(t.numel() * t.element_size() for t in (h_indptr, h_indices, hU, hV, hB))
     d2h = sum(t.numel() * t.element_size() for t in (hU, hV, hB)) + 16
-    steps = max(2, min(args.steps, 3))
+    steps = args.steps
 
     def one(e):
         hist, _ = engine.bpr_train_host(h_indptr.numpy(), h_indices.numpy(), W["n_items"], hU.numpy(), hV.numpy(),
@@ -756,7 +824,7 @@ def run_rank(W, engine, L, data, U, V, B, dev, world=1, over_ranks=lambda ms: ms
             "config": "BASELINE.json configs[4] on the trained bench model: all %d users (%d per rank) x %d items, k=%d, top-%d, "
                       "each user's train positives excluded" % (users_all, n_q, n_items, k, topk),
             "ms": round(ms, 3), "filled_frac_of_lists": round(filled, 4), "gpu_launches": launches,
-            "roofline": {"kernel": "rank_tc_kernel (tcgen05 fp16 -> f32) + finish + packs", "bound": "tensor", "achieved": round(tfl, 1),
+            "roofline": {"kernel": "rank_tc_kernel (wgmma fp16 -> f32) + finish + packs", "bound": "tensor", "achieved": round(tfl, 1),
                          "peak": tf_peak * world, "unit": "TFLOP/s", "frac": round(tfl / (tf_peak * world), 4), "peak_source": tf_src,
                          "note": "2*k*n_items flop per user over the WHOLE call (pack + tensor pass + exact finish), all ranks"},
             "cpu_baseline": cpu,
@@ -793,7 +861,7 @@ def reference_mf_ratings_per_s(rid, cid, val, n_users, n_items, k, budget_s=8.0)
     return epochs * len(val32) / secs, threads, epochs, secs
 
 
-def run_mf(W, engine, data, dev, world=1, over_ranks=lambda ms: ms, exchange="auto"):
+def run_mf(W, engine, data, dev, world=1, over_ranks=lambda ms: ms, exchange="auto", steps=3):
     """BASELINE.json configs[3]: MF ratings/s (b200_mf_epoch, Hogwild + atomic scatter), k = 128, on the rating list made
     of the model's interactions with synthetic ratings in {1..5}, stored by user (CSR order); every rank trains its
     shard, V / Bi are replicated and all-reduced once per epoch like BPR's."""
@@ -826,7 +894,6 @@ def run_mf(W, engine, data, dev, world=1, over_ranks=lambda ms: ms, exchange="au
     if world > 1:
         dist.barrier()
     sync, _ = checked_item_sync(sync, [V, Bi], world)
-    steps = 3
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()

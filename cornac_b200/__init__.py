@@ -1,4 +1,4 @@
-"""cornac_b200 -- B200 (sm_100a) implementation of Cornac's BPR / MF train-and-rank hot path.
+"""cornac_b200 -- H100 (sm_90a) implementation of Cornac's BPR / MF train-and-rank hot path.
 
     from cornac_b200 import BPR, MF        # drop-in for cornac.models.BPR / MF
     cornac.Experiment(eval_method=..., models=[BPR(k=64, ...)], metrics=[...]).run()

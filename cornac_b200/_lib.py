@@ -81,6 +81,7 @@ SGD_UNBOUNDED = 4
 BPR_NEG_WEIGHTED = 8
 BPR_LOSS_HINGE = 16
 BPR_BLOCKED = 32
+BPR_DETERMINISTIC = 64
 METRIC_NDCG, METRIC_PRECISION, METRIC_RECALL, METRIC_FMEASURE, METRIC_HIT, METRIC_NCRR = range(6)
 
 _lib = None
@@ -94,7 +95,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise B200Error(
             "libb200cornac.so not found at %s -- build it with `python -m cornac_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a).  There is no CPU fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)   # AttributeError if the header and the library disagree

@@ -1,9 +1,8 @@
-"""Build libb200cornac.so (sm_100a) in-tree with nvcc.
+"""Build libb200cornac.so (sm_90a, H100) in-tree with nvcc.
 
     python -m cornac_b200.build [--force]
 
-The shared library lands in cornac_b200/lib/ (git-ignored, shipped to the GPU box by
-gpurun).  nvcc cross-compiles without a GPU.  No torch involved: the library is a plain
+The shared library lands in cornac_b200/lib/ (git-ignored).  nvcc cross-compiles without a GPU.  No torch involved: the library is a plain
 C-ABI .so (include/b200cornac.h) loaded with ctypes.
 """
 import concurrent.futures
@@ -20,7 +19,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOSTCXX = os.environ.get("B200_HOSTCXX", "/usr/bin/g++")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-ccbin", HOSTCXX,
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall",
@@ -68,7 +67,7 @@ def build(force=False, verbose=False):
             if log:
                 print(log)
     if force or _stale(LIB, objs):
-        cmd = [NVCC, "-shared", "-ccbin", HOSTCXX, "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-ccbin", HOSTCXX, "-gencode", "arch=compute_90a,code=sm_90a",
                "-o", LIB] + objs + ["-lcuda"]
         p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if p.returncode != 0:

@@ -1,4 +1,4 @@
-// BPR SGD epochs for sm_100a.
+// BPR SGD epochs for sm_90a.
 //
 // Replaces BPR._fit_sgd (reference: cornac/models/bpr/recom_bpr.pyx:208-269) with
 //   * bpr_hogwild_kernel : throughput mode.  Persistent grid; every G-lane group draws its
@@ -24,8 +24,8 @@ namespace b200 {
 //   table  u64[slots]  open-addressing set of the keys (u << 32 | i), 4-slot (32-byte) buckets at
 //                      load <= 0.5: has_non_zero(u, j) is ONE 32-byte gather that can be issued
 //                      together with the factor rows, instead of a ~log2(deg)-deep dependent
-//                      binary search.  Costs 8 + ~21 bytes of HBM per interaction -- cheap on a
-//                      180 GB part, and it removes ~7 serialized memory round trips per sample.
+//                      binary search.  Costs 8 + ~21 bytes of HBM per interaction -- 3.6 GB for
+//                      125 M interactions on an 80 GB part, and it removes ~7 serialized memory round trips per sample.
 constexpr unsigned long long TABLE_EMPTY = ~0ull;
 
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x)
@@ -1069,19 +1069,15 @@ static int launch_hogwild(const BprParams& p, cudaStream_t st)
     constexpr int E = NPL * (VEC ? 4 : 1);
     const HogwildTune tune = read_tune();
     if constexpr (VEC && NPL == 1 && G >= 16) {
-        // one float4 per lane (k % 4 == 0, 52 <= k <= 128): rows staged in shared memory.  Measured on the configs[2] block
-        // (1.25 M x 1 M x 125 M, k = 128; profiles/r02_bpr.md): streamed, 2 samples in flight, 70.6 ms / epoch; 4 in
-        // flight 82.3 ms (the memory system, not the warp, is the queue); register-staged chunk kernel 81.3 ms.
-        // 16-lane groups (k <= 64, V L2-resident at configs[1]) stay on the chunk kernel: 24.2 ms vs 35.7 ms streamed x4.
+        // one float4 per lane (k % 4 == 0, 52 <= k <= 128): rows staged in shared memory, 2 samples in flight per group.
+        // 16-lane groups (k <= 64, V L2-resident at configs[1]) stay on the register-staged chunk kernel.
         if (tune.S == 0 && G >= 32) return launch_hogwild_stream<G, ATOMIC, 2, 4>(p, st, tune);
         if (tune.S == 2) return launch_hogwild_stream<G, ATOMIC, 2, 4>(p, st, tune);          // A/B: force the streamed kernels
         if (tune.S == 4) return launch_hogwild_stream<G, ATOMIC, 4, 4>(p, st, tune);
     }
     if constexpr (E <= 8) {
-        // measured on B200 (profiles/r01_bpr_scatter_experiments.txt): 16-lane groups run best two row-gathers
-        // ahead at 3 blocks/SM (4.14 vs 3.90 G samples/s on C2); 32-lane groups (k = 128: 512-byte rows, V beyond
-        // the L2 at 1 M items) gain nothing from the second slot but 15 % from a fourth resident block
-        // (60 registers; 1.55 vs 1.35 G updates/s on the configs[2] shard shape)
+        // 16-lane groups run two row-gathers ahead at 3 blocks/SM; 32-lane groups (k = 128: 512-byte rows, V beyond the
+        // L2 at 1 M items) one gather ahead at 4 resident blocks (60 registers).  B200_BPR_TUNE selects the others.
         if (tune.S == 0 || tune.S == 64) {       // (64 = the register-staged chunk kernel where the streamed one is the default)
             if (G >= 32) return launch_hogwild_chunk<G, NPL, VEC, ATOMIC, 4, 1>(p, st, tune);
             return launch_hogwild_chunk<G, NPL, VEC, ATOMIC, 3, 2>(p, st, tune);
@@ -1096,6 +1092,171 @@ static int launch_hogwild(const BprParams& p, cudaStream_t st)
     } else {
         return launch_hogwild_s<G, NPL, VEC, ATOMIC, 1, hogwild_min_blocks<NPL, VEC, 1>()>(p, st, tune);
     }
+}
+
+// ---------------------------------------------------------------------------------------
+// Deterministic throughput mode (B200_BPR_DETERMINISTIC): the epoch's samples run in rounds of at most DET_ROUND.  Every
+// sample of a round reads the factors as the previous round left them (bpr_det_grad_kernel writes nothing but the
+// accumulators), and the round's updates are summed in 2^-40 fixed point with integer atomics -- exact, so their order
+// does not matter -- before bpr_det_apply_kernel adds each touched element's sum once.  The result depends on the
+// seed and the sample law only, not on thread timing: a run repeats bit for bit.  A round is about as many samples as
+// the Hogwild kernels keep in flight, so the updates of a popular row are summed against a similar staleness.
+constexpr int64_t DET_ROUND = 16384;
+constexpr double DET_SCALE = 1099511627776.0;       // 2^40
+
+struct DetAcc {
+    unsigned long long* U;      // [n_users * k]  fixed-point sums of the round
+    unsigned long long* V;      // [n_neg * k]
+    unsigned long long* B;      // [n_neg]
+};
+
+// An update that is not finite or beyond the fixed-point range (|d| >= 2^22) cannot be summed: the element it belongs to
+// becomes NaN at once, so a diverging model shows NaN as under the Hogwild kernels instead of saturated sums.
+__device__ __forceinline__ void det_add(unsigned long long* a, float* x, float d)
+{
+    if (!(fabsf(d) < 4194304.f)) {
+        atomicExch(reinterpret_cast<unsigned int*>(x), 0x7fc00000u);
+        return;
+    }
+    const long long q = __double2ll_rn((double)d * DET_SCALE);
+    if (q) atomicAdd(a, (unsigned long long)q);
+}
+// the element's sum is taken (and cleared) by exactly one of the samples that touched it
+__device__ __forceinline__ void det_apply(unsigned long long* a, float* x)
+{
+    const long long q = (long long)atomicExch(a, 0ull);
+    if (q) atomicAdd(x, (float)((double)q * (1.0 / DET_SCALE)));
+}
+
+// (u, i) and j of epoch-local sample s: the law of the Hogwild kernels
+__device__ __forceinline__ void det_draw(const BprParams& p, int64_t s_local, int32_t& u, int32_t& i, int32_t& j)
+{
+    const uint64_t s = p.sample_base + (uint64_t)s_local;
+    const Philox4 r = philox4x32_10((uint32_t)s, (uint32_t)(s >> 32), p.epoch_lo, p.epoch_hi, p.seed_lo, p.seed_hi);
+    int64_t i_lo, i_len, j_lo, j_len;
+    law_ranges(p.law, s, i_lo, i_len, j_lo, j_len);
+    const int64_t ii = i_lo + (int64_t)range64(r.x, r.y, (uint64_t)i_len);
+    j = p.neg_weighted ? __ldg(p.pairs + range64(r.z, r.w, (uint64_t)p.nnz)).y
+                       : (int32_t)(j_lo + (int64_t)range64(r.z, r.w, (uint64_t)j_len));
+    const int2 pr = __ldg(p.pairs + ii);
+    u = pr.x;
+    i = pr.y;
+}
+
+// one warp per sample of [s_begin, s_end): skip test, score, z, the three row updates into the accumulators
+__global__ void __launch_bounds__(256) bpr_det_grad_kernel(const BprParams p, const DetAcc a, int64_t s_begin, int64_t s_end)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t s_loc = s_begin + ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
+    unsigned int n_correct = 0, n_skipped = 0;
+    if (s_loc < s_end) {
+        int32_t u, i, j;
+        det_draw(p, s_loc, u, i, j);
+        // has_non_zero(u, j)  (recom_bpr.pyx:241-243) = key (u, j) in the table
+        const uint64_t key = ((uint64_t)(uint32_t)u << 32) | (uint32_t)j;
+        uint64_t bb = mix64(key) & p.bucket_mask;
+        bool hit = false;
+        for (;;) {
+            const unsigned long long sl = (lane < 4) ? __ldg(p.table + 4 * bb + lane) : 0ull;
+            const unsigned h = __ballot_sync(0xffffffffu, lane < 4 && sl == key);
+            const unsigned f = __ballot_sync(0xffffffffu, lane == 3 && sl != TABLE_EMPTY);
+            if (h) { hit = true; break; }
+            if (!f) break;
+            bb = (bb + 1) & p.bucket_mask;
+        }
+        if (hit) {
+            n_skipped = 1;
+        } else {
+            const size_t k = (size_t)p.k;
+            const float* pu = p.U + (size_t)u * k;
+            const float* pi = p.V + (size_t)i * k;
+            const float* pj = p.V + (size_t)j * k;
+            float part = 0.f;
+            for (int e = lane; e < p.k; e += 32) part = fmaf(__ldcg(pu + e), __ldcg(pi + e) - __ldcg(pj + e), part);
+            const float bi = __ldcg(p.B + i), bj = __ldcg(p.B + j);
+            const float score = (bi - bj) + group_sum<32>(part);
+            float z = 1.f;
+            bool update = true;
+            if (p.hinge) {
+                if (score > 0.f) { n_correct = 1; update = false; }
+            } else {
+                z = bpr_z(score, p.exact_exp);
+                n_correct = (z < .5f);
+            }
+            if (update) {
+                const float lr = p.lr, reg = p.reg;
+                for (int e = lane; e < p.k; e += 32) {
+                    const float uf = __ldcg(pu + e), vi = __ldcg(pi + e), vj = __ldcg(pj + e);
+                    det_add(a.U + (size_t)u * k + e, p.U + (size_t)u * k + e, lr * (z * (vi - vj) - reg * uf));
+                    det_add(a.V + (size_t)i * k + e, p.V + (size_t)i * k + e, lr * (z * uf - reg * vi));
+                    det_add(a.V + (size_t)j * k + e, p.V + (size_t)j * k + e, lr * (-z * uf - reg * vj));
+                }
+                if (p.use_bias && lane == 0) {
+                    det_add(a.B + i, p.B + i, lr * (z - reg * bi));
+                    det_add(a.B + j, p.B + j, lr * (-z - reg * bj));
+                }
+            }
+        }
+    }
+    __shared__ unsigned int sh_stats[2];
+    if (threadIdx.x < 2) sh_stats[threadIdx.x] = 0;
+    __syncthreads();
+    if (lane == 0 && (n_correct | n_skipped)) {
+        atomicAdd(&sh_stats[0], n_correct);
+        atomicAdd(&sh_stats[1], n_skipped);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && (sh_stats[0] | sh_stats[1])) {
+        atomicAdd(p.stats + 0, (unsigned long long)sh_stats[0]);
+        atomicAdd(p.stats + 1, (unsigned long long)sh_stats[1]);
+    }
+}
+
+// one warp per sample of the same round: the summed updates of its rows, each element applied once
+__global__ void __launch_bounds__(256) bpr_det_apply_kernel(const BprParams p, const DetAcc a, int64_t s_begin, int64_t s_end)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t s_loc = s_begin + ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
+    if (s_loc >= s_end) return;
+    int32_t u, i, j;
+    det_draw(p, s_loc, u, i, j);
+    const size_t k = (size_t)p.k;
+    for (int e = lane; e < p.k; e += 32) {
+        det_apply(a.U + (size_t)u * k + e, p.U + (size_t)u * k + e);
+        det_apply(a.V + (size_t)i * k + e, p.V + (size_t)i * k + e);
+        det_apply(a.V + (size_t)j * k + e, p.V + (size_t)j * k + e);
+    }
+    if (p.use_bias && lane == 0) {
+        det_apply(a.B + i, p.B + i);
+        det_apply(a.B + j, p.B + j);
+    }
+}
+
+static int bpr_epoch_deterministic(const BprParams& p, int64_t n_users, cudaStream_t st)
+{
+    const int64_t round = p.max_groups < DET_ROUND ? p.max_groups : DET_ROUND;
+    const size_t nu = (size_t)n_users * p.k, nv = (size_t)p.n_neg * p.k;
+    const size_t bytes = (nu + nv + (size_t)p.n_neg) * sizeof(unsigned long long);
+    void* buf = nullptr;
+    B200_CUDA(cudaMallocAsync(&buf, bytes, st));
+    DetAcc a;
+    a.U = static_cast<unsigned long long*>(buf);
+    a.V = a.U + nu;
+    a.B = a.V + nv;
+    cudaError_t e = cudaMemsetAsync(buf, 0, bytes, st);      // the apply kernel leaves every sum it takes at zero
+    const unsigned grid = (unsigned)((round * 32 + 255) / 256);
+    for (int64_t s0 = 0; s0 < p.n_samples && e == cudaSuccess; s0 += round) {
+        const int64_t s1 = s0 + round < p.n_samples ? s0 + round : p.n_samples;
+        const unsigned g = (unsigned)(((s1 - s0) * 32 + 255) / 256);
+        bpr_det_grad_kernel<<<g < grid ? g : grid, 256, 0, st>>>(p, a, s0, s1);
+        bpr_det_apply_kernel<<<g < grid ? g : grid, 256, 0, st>>>(p, a, s0, s1);
+        ::b200::count_launch(2);
+        e = cudaGetLastError();
+    }
+    const cudaError_t f = cudaFreeAsync(buf, st);
+    if (e != cudaSuccess) return cuda_fail(e, "bpr_det_grad_kernel / bpr_det_apply_kernel", __FILE__, __LINE__);
+    B200_CUDA(f);
+    return B200_OK;
 }
 
 }  // namespace b200
@@ -1128,8 +1289,10 @@ extern "C" int b200_bpr_prepare(const int32_t* indptr, const int32_t* indices, i
     return B200_OK;
 }
 
-// Windows of the interaction list / blocks of the items such that one window's user rows and one block's item rows
-// (40 MB each) stay resident in the 126 MB L2 next to the hot positive rows; 1 / 1 when the matrix already fits.
+// Windows of the interaction list / blocks of the items of 40 MB of rows each, so that the rows one run of the epoch
+// touches are a small slice of the whole model instead of all of it; 1 / 1 when the matrix is within two parts.
+// The part size fixes the sample order of a blocked epoch; it was chosen for a 126 MB L2 and is kept on the H100's
+// 50 MB L2 (where only one part at a time can stay resident), so that a seed keeps drawing the same epochs.
 extern "C" int b200_bpr_block_plan(int64_t n_users, int64_t n_neg, int k, uint32_t* n_windows, uint32_t* n_blocks)
 {
     B200_REQUIRE(n_users >= 1 && n_neg >= 1 && k >= 1 && n_windows && n_blocks, "b200_bpr_block_plan: bad argument");
@@ -1206,6 +1369,7 @@ extern "C" int b200_bpr_epoch(const int32_t* pairs, const uint64_t* table, int64
     cudaStream_t st = (cudaStream_t)stream;
     const bool atomic = flags & B200_SGD_ATOMIC;
     p.exact_exp = (flags & B200_SGD_EXACT_EXP) ? 1 : 0;
+    if (flags & B200_BPR_DETERMINISTIC) return bpr_epoch_deterministic(p, n_users, st);
 #define CALL(G_, NPL_, VEC_)                                                                      \
     do {                                                                                          \
         const int rc = atomic ? launch_hogwild<G_, NPL_, VEC_, true>(p, st)                       \

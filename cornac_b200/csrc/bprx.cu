@@ -1,4 +1,4 @@
-// BPR siblings whose samples touch a THIRD item row: VEBPR and SBPR (SURVEY.md 8(f)-3), sm_100a.
+// BPR siblings whose samples touch a THIRD item row: VEBPR and SBPR (SURVEY.md 8(f)-3), sm_90a.
 //
 //   VEBPR  cornac/models/bpr/recom_vebpr.pyx:214-337  (u, i = purchased, v = viewed but not purchased, j = negative):
 //          three pairwise logistic terms i>j, i>v, v>j (weights 1, alpha, 1 - alpha), scores clipped to +-50, no item

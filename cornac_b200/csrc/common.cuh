@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the BPR / MF / score+rank hot path.
+// Shared helpers for the sm_90a kernels of the BPR / MF / score+rank hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// Biased matrix-factorisation SGD epochs for sm_100a.
+// Biased matrix-factorisation SGD epochs for sm_90a.
 //
 // Replaces one epoch of backend_cpu.fit_sgd (reference: cornac/models/mf/backend_cpu.pyx:58-83):
 //   * mf_hogwild_kernel : every G-lane group owns one rating at a time (grid-stride over the

@@ -1,4 +1,4 @@
-// Tensor-core fused score + top-k for sm_100a (tcgen05 / TMEM / TMA bulk copies).
+// Tensor-core fused score + top-k for sm_90a (wgmma / TMA bulk copies / mbarrier).
 //
 // Replaces, for a batch of users, the reference's per-user pipeline
 //     fast_dot(U[u], V, bias)            cornac/utils/fast_dot.pyx:40-43
@@ -6,8 +6,8 @@
 // driven once per test user by ranking_eval (cornac/eval_methods/base_method.py:177-220).
 //
 // Plan of one call (users are processed in chunks so the candidate lists stay small):
-//   1. pack   V (and the chunk's U rows) to fp16 in the UMMA "K-major, no swizzle" core-matrix
-//             layout, tile by tile, so that one tile is ONE contiguous cp.async.bulk (UBLKCP).  Both
+//   1. pack   V (and the chunk's U rows) to fp16 in the GMMA "K-major, no swizzle" core-matrix
+//             layout, tile by tile, so that one tile is ONE contiguous cp.async.bulk.  Both
 //             sides are first multiplied by a power of two (exact) that brings their largest element
 //             to [2^13, 2^14), so the fp16 range is never left and the rounding error is the 2^-11
 //             relative one (8x smaller than bf16's: 8x tighter candidate filter); an extra K slice
@@ -15,15 +15,14 @@
 //             MMA adds it; per-row norms give the rigorous error bound eps(u) ~ 2^-10 |u| max|v|
 //             (+ subnormal, accumulation and base terms, see `row_eps`) of the fp16 pass;
 //   2. rank_tc_kernel  persistent, one CTA per SM, warp-specialised:
-//               warp 0   TMA producer: U tile once per 128 users, V tiles (256 items) through a
-//                        ring of smem stages released by tcgen05.commit (mbarriers)
-//               warp 1   one elected thread issues tcgen05.mma (M=128, N=256, K=16 per
-//                        instruction, fp16 x fp16 -> f32) into a double-buffered TMEM accumulator
-//               warp 2   TMEM allocation
-//               warps 4-11 epilogue: tcgen05.ld the accumulator (one (user row, 128-column half)
-//                        per thread), keep every score above the row's running threshold in the
-//                        thread's candidate list; the threshold is raised (never above the
-//                        approximate k-th best minus 2*eps) by lock-step scans of the lists
+//               warp 0   TMA producer: U tile once per 128 users, V stages (128 items, half of a
+//                        packed 256-item tile) through a ring of smem stages released by the consumers
+//               warps 4-11  two consumer warpgroups, each owning 64 user rows: wgmma (M=64, N=128,
+//                        K=16 per instruction, fp16 x fp16 -> f32 in registers), then the accumulator is
+//                        passed through shared memory so that every thread owns one (user row, 64-column
+//                        strip); it keeps every score above the row's running threshold in the thread's
+//                        candidate list; the threshold is raised (never above the approximate k-th best
+//                        minus 2*eps) by lock-step scans of the lists
 //   3. rank_tc_finish_kernel  per row: exact re-score of the candidates (the f64-accumulated
 //             arithmetic of score_batch_kernel), total order (score desc, id asc), top-k.
 // The tensor pass only NOMINATES: every item whose exact score can reach the top-k is provably
@@ -38,21 +37,21 @@ namespace b200 {
 
 namespace tc {
 
-constexpr int TM = 128;            // users per tile  (UMMA M)
-constexpr int TN = 256;            // items per stage (UMMA N)
-// The accumulator columns are split into ST strips (2 or 4); 4 epilogue warps (one per TMEM lane quarter) per strip:
-//   ST = 2: 12 warps (TMA, MMA, TMEM-alloc, idle, 8 x epilogue), strips of 128 columns, lists of 1024 entries
-//   ST = 4: 20 warps (16 x epilogue), strips of 64 columns, lists of 512 entries
-constexpr int MAX_ST = 4;
-__host__ __device__ constexpr int threads_for(int st) { return 128 + 128 * st; }
-__host__ __device__ constexpr int cap_for(int st) { return 2048 / st; }
+constexpr int TM = 128;            // users per tile (two warpgroups of M = 64)
+constexpr int TN = 256;            // items per packed V tile (the padding unit of the item side)
+constexpr int SN = 128;            // items per pipeline stage (wgmma N): half of a packed tile, itself a contiguous tile image
+constexpr int ST = 2;              // column strips of a stage: 64 columns per epilogue thread
+constexpr int STRIP_N = SN / ST;
+constexpr int EPI_WARPS = 4 * ST;  // 8 consumer warps = 2 warpgroups
+constexpr int THREADS = 128 + 32 * EPI_WARPS;     // warps 0-3: TMA producer (warp 0) + idle, warps 4-11: consumers
+constexpr int LDT = SN + 8;        // row stride (floats) of the accumulator hand-off: conflict-free fragment stores
+constexpr int MAX_ST = 4;          // per-row slots of row_cnt / row_flag / row_tau (the finish reads `strips` of them)
 constexpr int KX = 16;             // extra K slice carrying the item base: U gets (cA, cA, 1, 0...), V gets (hi, lo, pad ? -inf : 0, 0...)
-constexpr int CAP = 1024;          // candidate-list capacity of a strip list at ST = 2 (cap_for(ST) in general)
+constexpr int CAP = 1024;          // candidate-list capacity of one (row, strip) list
 constexpr int NB = 32;             // score bins of a threshold raise (one pass over the list, counters in shared memory)
 constexpr int MAX_TOPK = 256;
 constexpr int MAX_KP = 128 + KX;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr int CHUNK_TILES = 148 * 4;   // user tiles per chunk
+constexpr int CHUNK_TILES = 132 * 4;   // user tiles per chunk (4 waves of the H100's 132 SMs)
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -83,8 +82,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
             : "memory");
     } while (!ok);
 }
-// same, for the two single-thread roles (TMA producer, MMA issuer): back off between polls so the
-// spinning lane does not steal issue slots from the epilogue warps that share its scheduler
+// same, for the single-thread TMA producer: back off between polls so the spinning lane does not steal issue slots
+// from the consumer warps that share its scheduler
 __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity)
 {
     const uint32_t addr = smem_u32(bar);
@@ -107,157 +106,62 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols)
+// named barrier of `n` threads
+__device__ __forceinline__ void named_sync(int id, int n)
 {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 columns of f32: thread t of the warp receives row (lane base + t), columns c..c+31
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-// wait for the outstanding tcgen05.ld; the registers are passed through the asm so that no use of
-// them can be scheduled above the wait
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[32])
-{
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                   "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-                   "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :: "memory");
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
 
-// ---- CTA-pair (cta_group::2) forms: two CTAs of a cluster, one per SM of a TPC, run ONE MMA of M = 256 together: each
-// supplies its own 128 rows of A and HALF of the B tile from its own shared memory, each receives its 128 rows of D in
-// its own TMEM.  The instruction, the commits and the TMEM allocation name the pair explicitly.
-__device__ __forceinline__ uint32_t cluster_ctarank()
-{
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_smem_addr` in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t rank)
-{
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr)
-{
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// The accumulator hand-back of the follower's (and the leader's) epilogue warps.  A release at cluster scope compiles to
-// MEMBAR.ALL.GPU + ERRBAR, which waits for every outstanding global store of the warp -- the candidate appends: 31 % of
-// all stall samples of the pair kernel (profiles/r02_rank_tc_pair_membar.md).  Nothing written to MEMORY is handed over
-// here: the consumer (the MMA issuer) only needs the TMEM reads of this warp to have completed, which tcgen05.wait::ld +
-// tcgen05.fence::before_thread_sync order before the arrive; so the arrive itself is relaxed.
-__device__ __forceinline__ void mbar_arrive_remote_relaxed(uint32_t cluster_addr)
-{
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait on a barrier that threads of the PEER CTA arrive on (cluster-scope acquire), with back-off
-__device__ __forceinline__ void mbar_wait_cluster_backoff(uint64_t* bar, uint32_t parity)
-{
-    const uint32_t addr = smem_u32(bar);
-    uint32_t ok;
-    for (;;) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(addr), "r"(parity)
-            : "memory");
-        if (ok) break;
-        __nanosleep(20);
-    }
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* dst_smem, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive (once the MMAs issued so far have retired) on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((unsigned short)3) : "memory");
-}
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_NONE ("interleaved" core matrices):
+// GMMA shared-memory descriptor, K-major, no swizzle ("interleaved" core matrices):
 // a core matrix is 8 rows x 16 bytes stored as 128 contiguous bytes; LBO = byte distance between
 // the two K-halves (16-byte chunks) of one K=16 instruction, SBO = byte distance between 8-row
-// groups (cute::UMMA::SmemDescriptor, "((8,n),2):((1,SBO),LBO)" in 16-byte units).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
+// groups ("((8,n),2):((1,SBO),LBO)" in 16-byte units).
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;          // descriptor version (sm_100)
-    return d;                        // base_offset = 0, lbo_mode = 0, layout_type = SWIZZLE_NONE (0)
+    return d;                        // base_offset = 0, layout_type (bits 62-63) = no swizzle
 }
-// instruction descriptor: D = f32 (bit 4), A = B = fp16 (format fields 7-9 / 10-12 = 0), both K-major, M x N
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, fp16 operands from shared memory (both K-major), f32 accumulators in
+// registers: thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1)
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
 }
 
-// V-tile ring depth that fits next to the U tile in 200 KB of shared memory (2..4); the rest holds barriers,
-// thresholds and the pair-exchange area
-// (a CTA of a pair stages only its half of every V tile: TN / cg items)
-__host__ __device__ __forceinline__ int num_stages(int kp, int st, int cg)
+// shared memory of rank_tc_kernel besides the U tile and the V ring: the accumulator hand-off of the two warpgroups,
+// the barriers, the per-row threshold / exchange slots and the score-bin counters of a raise
+constexpr int SMEM_FIXED = 2 * 64 * LDT * 4 + 16 * 8 + ST * TM * 8 + ST * TM * 4 * 4 + ST * NB * TM * 2 + 1024;
+constexpr int SMEM_MAX = 227 * 1024;   // opt-in shared memory per block on sm_90
+
+// V-stage ring depth that fits next to the U tile and the fixed part (2..4)
+__host__ __device__ __forceinline__ int num_stages(int kp)
 {
-    const int budget = (st == 4 ? 180 : 200) * 1024 - TM * kp * 2;
-    int ns = budget / ((TN / cg) * kp * 2);
+    const int budget = SMEM_MAX - SMEM_FIXED - TM * kp * 2;
+    int ns = budget / (SN * kp * 2);
     return ns > 4 ? 4 : (ns < 2 ? 2 : ns);
 }
 
@@ -457,8 +361,7 @@ struct RankTcParams {
     int* __restrict__ row_flag;            // [n_ut * TM][MAX_ST] 1 = list overflow -> exact path
     float* __restrict__ row_tau;           // [n_ut * TM][MAX_ST] final filter tau - 2 eps of the strip (scaled units): the finish drops entries below the row's largest
     float* __restrict__ dump;              // debug: dense approximate scores [n_ut*TM][n_it*TN] or null
-    int debug;                             // B200_RANK_DEBUG: timing only: 1 = epilogue hands the accumulators straight back, 2 = tcgen05.ld only;
-                                           // 8 = screening only (no candidate is listed);
+    int debug;                             // B200_RANK_DEBUG: timing only: 8 = screening only (no candidate is listed);
                                            // 4 = raise schedule with ratio 1.41 instead of 2 (results stay exact)
 };
 
@@ -681,13 +584,7 @@ __device__ __forceinline__ void raise_threshold(RowState& st, int K, float eps2,
     }
 }
 
-// three-input maximum (FMNMX3, sm_100+)
-__device__ __forceinline__ float fmax3(float a, float b, float c)
-{
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
-}
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // append the scores of one group of four that pass the filter to the calling lane's list
 __device__ __noinline__ unsigned long long* append4(unsigned long long* wp, float tau_f, float s0, float s1, float s2,
@@ -715,7 +612,7 @@ __device__ __forceinline__ void epilogue_chunk(uint32_t (&r)[32], RowState& st, 
             for (int x = 0; x < 32; ++x) dump_row[id0 + x] = __uint_as_float(r[x]) * invS;
         }
     } else {
-    // phase 1: maxima of the eight groups of four (three-input max: 2 instructions per group) and of the whole
+    // phase 1: maxima of the eight groups of four and of the whole
     // chunk; ONE vote decides whether any of the warp's 32 x 32 scores passes the filter at all
     float m[8];
 #pragma unroll
@@ -739,150 +636,79 @@ __device__ __forceinline__ void epilogue_chunk(uint32_t (&r)[32], RowState& st, 
     }
 }
 
-// CG = 1: one CTA per SM works alone on 128-user tiles.  CG = 2: the two CTAs of a cluster (one TPC) work on a PAIR of
-// user tiles with cta_group::2 MMAs (M = 256): each CTA stages its own U tile and only HALF of every V tile, so the item
-// matrix crosses the L2 -> SM fabric once per 256 users instead of once per 128 (the single-CTA kernel is bound by
-// exactly that traffic: 148 CTAs x 74 KB per stage ~ 10 TB/s out of L2) and the tensor pipe reads half as many B bytes
-// from each SM's shared memory.  Barrier protocol of the pair (rank 0 = leader, the only MMA issuer):
-//   full[s], u_full      local, armed by the CTA's own TMA producer
-//   pair_full[s], pair_u leader's, 2 arrivals: each CTA's relay thread (warp 3) forwards "my half / my U tile landed"
-//   empty[s], u_empty, acc_full[a]   local in BOTH CTAs, signalled by the leader's tcgen05.commit (multicast)
-//   acc_empty[a]         leader's, 2 x EPI_WARPS arrivals: the follower's epilogue warps arrive remotely
+// One CTA per SM works on 128-user tiles; per tile it streams the packed item side in stages of SN = 128 items.
+// Barrier protocol:
+//   full[s], u_full      armed by the TMA producer (expect_tx), completed by the bulk copies
+//   empty[s], u_empty    EPI_WARPS arrivals: every consumer warp, once its wgmma reading the stage (the U tile) retired
+// Each consumer warpgroup computes its 64 rows x SN columns with wgmma into registers, passes them through its own
+// shared-memory block (row stride LDT) and reads back one (row, 64-column strip) per thread: warp w of warpgroup g owns
+// rows 64 g + 32 (w & 1) + lane, strip w >> 1 -- the 32-row quarter q = 2 g + (w & 1) of the tile, as in the list layout
+// the finish kernels read.
 // DBG: the timing-experiment switches (B200_RANK_DEBUG) are compiled into a separate instantiation; the production kernel
-// carries none of their branches (the stage loop is sensitive to every instruction and register, profiles/r02_rank_tc.md).
-template <bool DUMP, int ST, int CG, bool DBG = false>
-__global__ void __launch_bounds__(threads_for(ST), 1) rank_tc_kernel(const RankTcParams p)
+// carries none of their branches.
+template <bool DUMP, bool DBG = false>
+__global__ void __launch_bounds__(THREADS, 1) rank_tc_kernel(const RankTcParams p)
 {
     const int dbg = DBG ? p.debug : 0;
-    constexpr int EPI_WARPS = 4 * ST;
-    constexpr int STRIP_N = TN / ST;
-    constexpr int CAP_T = cap_for(ST);
+    constexpr int CAP_T = CAP;
     constexpr int TRIGGER = CAP_T / 2;
     extern __shared__ __align__(1024) uint8_t smem[];
     const int kp = p.kp;
-    const uint32_t u_bytes = TM * kp * 2, v_bytes = TN * kp * 2, v_part = v_bytes / CG;
-    const int NS = num_stages(kp, ST, CG);
+    const uint32_t u_bytes = TM * kp * 2, s_bytes = SN * kp * 2;
+    const int NS = num_stages(kp);
+    const int n_st = p.n_it * (TN / SN);          // stages per user tile
     uint8_t* sU = smem;
     uint8_t* sV = sU + u_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + (size_t)NS * v_part);
-    uint64_t* full = bars;            // [NS]  V tile (part) landed          TMA -> MMA (CG = 2: -> relay)
-    uint64_t* empty = bars + 4;       // [NS]  MMAs reading the tile retired MMA commit -> TMA
+    float* sT = reinterpret_cast<float*>(sV + (size_t)NS * s_bytes);          // [2 warpgroups][64 rows][LDT]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sT + 2 * 64 * LDT);
+    uint64_t* full = bars;            // [NS]  V stage landed                TMA -> consumers
+    uint64_t* empty = bars + 4;       // [NS]  wgmma reading the stage retired  consumers -> TMA
     uint64_t* u_full = bars + 8;      // U tile landed
-    uint64_t* u_empty = bars + 9;     // all MMAs of the user tile retired
-    uint64_t* acc_full = bars + 10;   // [2] accumulator ready               MMA commit -> epilogue
-    uint64_t* acc_empty = bars + 12;  // [2] accumulator drained             epilogue warps -> MMA
-    uint64_t* pair_full = bars + 14;  // [NS] CG = 2, leader: both halves of the V tile landed
-    uint64_t* pair_u = bars + 18;     // CG = 2, leader: both U tiles landed
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 22);
+    uint64_t* u_empty = bars + 9;     // all wgmma of the user tile retired
     // [ST strips][TM rows] last published row threshold, tagged with the tile it belongs to: (tile << 32) | f32 bits
-    unsigned long long* tau_share = reinterpret_cast<unsigned long long*>(bars + 24);
+    unsigned long long* tau_share = reinterpret_cast<unsigned long long*>(bars + 16);
     // [ST strips][TM rows][4] list length and score range exchanged by the ST threads of a row
-    int* pair_share = reinterpret_cast<int*>(bars + 24 + ST * TM);
+    int* pair_share = reinterpret_cast<int*>(tau_share + ST * TM);
     // [ST strips][NB bins][TM rows] per-thread score-bin counters of a threshold raise
     unsigned short* hist_share = reinterpret_cast<unsigned short*>(pair_share + ST * TM * 4);
-    // The V ring is released by the tensor pipe alone, so the TMA producer runs NS tiles ahead of the
-    // MMAs whatever the epilogue does; the epilogue only hands the TMEM accumulators back.
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t cta_rank = CG == 2 ? cluster_ctarank() : 0u;
-    const int first_group = (int)(blockIdx.x / CG), n_groups = (int)(gridDim.x / CG);   // group = CTA (CG = 1) or CTA pair
-    const int n_gt = (p.n_ut + CG - 1) / CG;                                            // tile groups of the chunk
-
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NS; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); mbar_init(pair_full + s, 2); }
+        for (int s = 0; s < NS; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, EPI_WARPS); }
         mbar_init(u_full, 1);
-        mbar_init(u_empty, 1);
-        mbar_init(pair_u, 2);
-        for (int a = 0; a < 2; ++a) { mbar_init(acc_full + a, 1); mbar_init(acc_empty + a, EPI_WARPS * CG); }
+        mbar_init(u_empty, EPI_WARPS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        if (CG == 2) tmem_alloc2(tmem_ptr, TMEM_COLS); else tmem_alloc(tmem_ptr, TMEM_COLS);
-    }
-    tc_fence_before();
-    if (CG == 2) cluster_sync_all(); else __syncthreads();      // barriers of BOTH CTAs are initialised before any remote arrive
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
+    __syncthreads();
 
     if (warp == 0) {
         // ===================== TMA producer =====================
         if (lane == 0) {
             uint32_t it_global = 0, tile_no = 0;
-            for (int gt = first_group; gt < n_gt; gt += n_groups, ++tile_no) {
-                const int ut = gt * CG + (int)cta_rank;          // (an odd chunk's last pair: a zero tile, packed as padding)
+            for (int ut = blockIdx.x; ut < p.n_ut; ut += gridDim.x, ++tile_no) {
                 if (tile_no > 0) mbar_wait_backoff(u_empty, (tile_no - 1) & 1);
                 mbar_expect_tx(u_full, u_bytes);
                 bulk_g2s(sU, p.Upack + (size_t)ut * u_bytes, u_bytes, u_full);
-                for (int it = 0; it < p.n_it; ++it, ++it_global) {
+                for (int it = 0; it < n_st; ++it, ++it_global) {
                     const int s = it_global % NS;
                     const uint32_t round = it_global / NS;
                     if (round > 0) mbar_wait_backoff(empty + s, (round - 1) & 1);
-                    mbar_expect_tx(full + s, v_part);
-                    bulk_g2s(sV + (size_t)s * v_part, p.Vpack + (size_t)it * v_bytes + (size_t)cta_rank * v_part, v_part, full + s);
+                    mbar_expect_tx(full + s, s_bytes);
+                    bulk_g2s(sV + (size_t)s * s_bytes, p.Vpack + (size_t)it * s_bytes, s_bytes, full + s);
                 }
-            }
-        }
-    } else if (warp == 3) {
-        // ===================== relay (CTA pairs): "my part landed" -> the leader's pair barriers =====================
-        if (CG == 2 && lane == 0) {
-            const uint32_t r_pair_u = mapa_u32(smem_u32(pair_u), 0);
-            uint32_t it_global = 0, tile_no = 0;
-            for (int gt = first_group; gt < n_gt; gt += n_groups, ++tile_no) {
-                mbar_wait_backoff(u_full, tile_no & 1);
-                mbar_arrive_remote(r_pair_u);
-                for (int it = 0; it < p.n_it; ++it, ++it_global) {
-                    const int s = it_global % NS;
-                    mbar_wait_backoff(full + s, (it_global / NS) & 1);
-                    mbar_arrive_remote(mapa_u32(smem_u32(pair_full + s), 0));
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (of a pair: the leader only) =====================
-        if (lane == 0 && cta_rank == 0) {
-            const uint32_t idesc = umma_idesc_f16(TM * CG, TN);
-            const uint32_t lbo = 128, sbo = (uint32_t)(kp >> 3) * 128;
-            uint32_t it_global = 0, tile_no = 0;
-            for (int gt = first_group; gt < n_gt; gt += n_groups, ++tile_no) {
-                if (CG == 2) mbar_wait_cluster_backoff(pair_u, tile_no & 1); else mbar_wait_backoff(u_full, tile_no & 1);
-                for (int it = 0; it < p.n_it; ++it, ++it_global) {
-                    const int s = it_global % NS;
-                    const int acc = it_global & 1;
-                    const uint32_t acc_round = it_global >> 1;
-                    if (CG == 2) mbar_wait_cluster_backoff(pair_full + s, (it_global / NS) & 1);
-                    else mbar_wait_backoff(full + s, (it_global / NS) & 1);
-                    if (acc_round > 0) {
-                        if (CG == 2) mbar_wait_cluster_backoff(acc_empty + acc, (acc_round - 1) & 1);
-                        else mbar_wait_backoff(acc_empty + acc, (acc_round - 1) & 1);
-                    }
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(sU), b_addr = smem_u32(sV + (size_t)s * v_part);
-                    const uint32_t d_tmem = tmem_base + (uint32_t)acc * TN;
-                    for (int ks = 0; ks < (kp >> 4); ++ks) {
-                        const uint64_t ad = umma_desc(a_addr + ks * 256, lbo, sbo);
-                        const uint64_t bd = umma_desc(b_addr + ks * 256, lbo, sbo);
-                        if (CG == 2) umma_f16_pair(d_tmem, ad, bd, idesc, ks > 0 ? 1u : 0u);
-                        else umma_f16(d_tmem, ad, bd, idesc, ks > 0 ? 1u : 0u);
-                    }
-                    if (CG == 2) {
-                        umma_commit_pair(empty + s);       // both CTAs' stages may be refilled once these MMAs retire
-                        umma_commit_pair(acc_full + acc);  // both CTAs' halves of the accumulator are complete
-                    } else {
-                        umma_commit(empty + s);
-                        umma_commit(acc_full + acc);
-                    }
-                }
-                if (CG == 2) umma_commit_pair(u_empty); else umma_commit(u_empty);
             }
         }
     } else if (warp >= 4) {
-        // ===================== epilogue: one (user row, column strip) per thread =====================
-        const int q = warp & 3;                          // TMEM lane quarter == warp % 4
-        const int half = (warp - 4) >> 2;                // column strip: columns [half * STRIP_N, (half + 1) * STRIP_N)
-        uint32_t it_global = 0;
-        const uint32_t r_acc_empty = CG == 2 ? mapa_u32(smem_u32(acc_empty), 0) : 0u;    // the leader's accumulator hand-back barriers
-        for (int gt = first_group; gt < n_gt; gt += n_groups) {
-            const int ut = gt * CG + (int)cta_rank;
+        // ===================== consumers: wgmma, then one (user row, column strip) per thread =====================
+        const int g = (warp - 4) >> 2;                   // warpgroup: rows [64 g, 64 g + 64) of the tile
+        const int w = warp & 3;                          // warp of the warpgroup
+        const int q = 2 * g + (w & 1);                   // 32-row quarter of the tile
+        const int half = w >> 1;                         // column strip: columns [half * STRIP_N, (half + 1) * STRIP_N)
+        float* tg = sT + (size_t)g * 64 * LDT;
+        const uint32_t lbo = 128, sbo = (uint32_t)(kp >> 3) * 128;
+        const uint32_t a_base = smem_u32(sU) + (uint32_t)g * 8 * sbo;      // the warpgroup's 64 rows = 8 core-matrix rows
+        uint32_t it_global = 0, tile_no = 0;
+        for (int ut = blockIdx.x; ut < p.n_ut; ut += gridDim.x, ++tile_no) {
             const int64_t row = (int64_t)ut * TM + q * 32 + lane;
             const bool valid = row < p.n_rows;
             const float un = valid ? p.unorm[row] : 0.f;
@@ -921,75 +747,64 @@ __global__ void __launch_bounds__(threads_for(ST), 1) rank_tc_kernel(const RankT
             int flag = 0;
             float* dump_row = DUMP ? p.dump + (size_t)(valid ? row : 0) * ((size_t)p.n_it * TN) : nullptr;
             int next_sched = 2;
-            for (int it = 0; it < p.n_it; ++it, ++it_global) {
-                const int acc = it_global & 1;
-                mbar_wait(acc_full + acc, (it_global >> 1) & 1);
-                tc_fence_after();
-                const int32_t item0 = it * TN + half * STRIP_N;
-                const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TN + half * STRIP_N);
+            mbar_wait(u_full, tile_no & 1);
+            for (int it = 0; it < n_st; ++it, ++it_global) {
+                const int s = it_global % NS;
+                mbar_wait(full + s, (it_global / NS) & 1);
+                const uint32_t b_base = smem_u32(sV + (size_t)s * s_bytes);
+                float acc[64];                              // set here so that it is dead during the screening
+#pragma unroll
+                for (int x = 0; x < 64; ++x) acc[x] = 0.f;
+                __syncwarp();
+                wgmma_fence();
+                for (int ks = 0; ks < (kp >> 4); ++ks)
+                    wgmma_m64n128k16(acc, gmma_desc(a_base + ks * 256, lbo, sbo), gmma_desc(b_base + ks * 256, lbo, sbo),
+                                     ks > 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait_all();
+                __syncwarp();
+                if (lane == 0) {
+                    mbar_arrive(empty + s);                 // the stage may be refilled
+                    if (it == n_st - 1) mbar_arrive(u_empty);
+                }
+                // accumulator fragments -> the warpgroup's block -> one 64-column row strip per thread
+                named_sync(5 + g, 128);                     // every thread has read the previous stage's block
+                {
+                    const int fr = 16 * w + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+                    for (int j = 0; j < SN / 8; ++j) {
+                        *reinterpret_cast<float2*>(tg + (size_t)fr * LDT + 8 * j + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                        *reinterpret_cast<float2*>(tg + (size_t)(fr + 8) * LDT + 8 * j + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                    }
+                }
+                named_sync(5 + g, 128);
                 uint32_t r0[32], r1[32];
-                if (dbg & 1) {                 // timing experiment: MMA / TMA feed rate without the screening
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) { if (CG == 2) mbar_arrive_remote_relaxed(r_acc_empty + 8 * acc); else mbar_arrive(acc_empty + acc); }
-                    continue;
-                }
-                if (dbg & 2) {                 // timing experiment: TMEM drain rate (tcgen05.ld only, no screening)
-                    uint32_t acc_or = 0;
+                {
+                    const float4* src = reinterpret_cast<const float4*>(tg + (size_t)((w & 1) * 32 + lane) * LDT + half * STRIP_N);
 #pragma unroll
-                    for (int c0 = 0; c0 < STRIP_N; c0 += 32) {
-                        tmem_ld32_issue(t0 + c0, r0);
-                        tmem_ld_wait(r0);
-                        acc_or |= r0[0] ^ r0[31];
+                    for (int x = 0; x < 8; ++x) {
+                        const float4 v0 = src[x], v1 = src[8 + x];
+                        r0[4 * x] = __float_as_uint(v0.x); r0[4 * x + 1] = __float_as_uint(v0.y);
+                        r0[4 * x + 2] = __float_as_uint(v0.z); r0[4 * x + 3] = __float_as_uint(v0.w);
+                        r1[4 * x] = __float_as_uint(v1.x); r1[4 * x + 1] = __float_as_uint(v1.y);
+                        r1[4 * x + 2] = __float_as_uint(v1.z); r1[4 * x + 3] = __float_as_uint(v1.w);
                     }
-                    if (acc_or == 0x12345u) flag = 1;          // keep the loads alive
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) { if (CG == 2) mbar_arrive_remote_relaxed(r_acc_empty + 8 * acc); else mbar_arrive(acc_empty + acc); }
-                    continue;
                 }
-                // The accumulator goes back to the tensor pipe as soon as this warp's columns are in REGISTERS -- before the
-                // screening of the last 64 of them, whose data-dependent appends then run off the MMA's critical path
-                // (with 64-column strips: all of the screening).
+                const int32_t item0 = it * SN + half * STRIP_N;
                 st.wp = st.list + (size_t)st.cnt * 32;
-                auto hand_back = [&]() {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) { if (CG == 2) mbar_arrive_remote_relaxed(r_acc_empty + 8 * acc); else mbar_arrive(acc_empty + acc); }
-                };
-                if constexpr (STRIP_N == 64) {
-                    tmem_ld32_issue(t0, r0);
-                    tmem_ld32_issue(t0 + 32, r1);
-                    tmem_ld_wait(r0);
-                    tmem_ld_wait(r1);
-                    hand_back();
-                    epilogue_chunk<DUMP>(r0, st, item0, dump_row, valid, invS);
-                    epilogue_chunk<DUMP>(r1, st, item0 + 32, dump_row, valid, invS);
-                } else {
-                    tmem_ld32_issue(t0, r0);
-                    tmem_ld_wait(r0);
-#pragma unroll
-                    for (int c0 = 0; c0 < STRIP_N; c0 += 64) {
-                        tmem_ld32_issue(t0 + c0 + 32, r1);                    // in flight while r0 is processed
-                        epilogue_chunk<DUMP>(r0, st, item0 + c0, dump_row, valid, invS);
-                        tmem_ld_wait(r1);
-                        if (c0 + 64 < STRIP_N) tmem_ld32_issue(t0 + c0 + 64, r0); else hand_back();
-                        epilogue_chunk<DUMP>(r1, st, item0 + c0 + 32, dump_row, valid, invS);
-                        if (c0 + 64 < STRIP_N) tmem_ld_wait(r0);
-                    }
-                }
+                epilogue_chunk<DUMP>(r0, st, item0, dump_row, valid, invS);
+                epilogue_chunk<DUMP>(r1, st, item0 + 32, dump_row, valid, invS);
                 st.cnt = (int)((st.wp - st.list) >> 5);
                 if (!DUMP) {
-                    // Raise schedule: after stages 2, 4, 8, 16, ... for EVERY warp at once (a raise stalls the
-                    // accumulator hand-off; doing it in all warps at the same stage costs one stall instead of
-                    // eight), plus whenever a list reaches TRIGGER.  Between two scheduled raises a list gains
-                    // ~K ln 2 entries, so the lists stay short.  A list grows by at most HALF_N entries per
-                    // stage: keep cnt <= CAP - HALF_N.
+                    // Raise schedule: after stages 2, 4, 8, 16, ... for EVERY warp at once (doing it in all warps at the
+                    // same stage costs one stall instead of eight), plus whenever a list reaches TRIGGER.  Between two
+                    // scheduled raises a list gains ~K ln 2 entries, so the lists stay short.  A list grows by at most
+                    // STRIP_N entries per stage: keep cnt <= CAP - STRIP_N.
                     const int done = it + 1;
-                    // ... and once more after the LAST stage: the lists then hold ~K ln(n_it / last raise) entries above a
+                    // ... and once more after the LAST stage: the lists then hold ~K ln(n_st / last raise) entries above a
                     // stale threshold, every one of which the finish kernel would re-score exactly (a 512-byte gather from V
                     // per candidate: the finish is HBM-bound on those gathers)
-                    const bool scheduled = (done == next_sched && !(dbg & 64)) || done == p.n_it;      // bit 64: timing experiment, final raise only
+                    const bool scheduled = (done == next_sched && !(dbg & 64)) || done == n_st;      // bit 64: timing experiment, final raise only
                     if (scheduled) {               // geometric schedule, ratio 2 (or ~1.41 with debug bit 4)
                         const int grown = (dbg & 4) ? (done * 181) >> 7 : done * 2;
                         next_sched = grown > done ? grown : done + 1;
@@ -1010,12 +825,6 @@ __global__ void __launch_bounds__(threads_for(ST), 1) rank_tc_kernel(const RankT
                 p.row_tau[row * MAX_ST + half] = st.tau_f;
             }
         }
-    }
-
-    tc_fence_before();
-    if (CG == 2) cluster_sync_all(); else __syncthreads();      // no CTA leaves while its peer may still signal into it
-    if (warp == 2) {
-        if (CG == 2) tmem_dealloc2(tmem_base, TMEM_COLS); else tmem_dealloc(tmem_base, TMEM_COLS);
     }
 }
 
@@ -1400,7 +1209,6 @@ static Layout make_layout(int64_t n_q, int64_t n_items, int k)
     L.n_it = (n_items + TN - 1) / TN;
     int64_t n_ut = (n_q + TM - 1) / TM;
     L.chunk_ut = n_ut < CHUNK_TILES ? n_ut : CHUNK_TILES;
-    L.chunk_ut = (L.chunk_ut + 1) & ~(int64_t)1;     // CTA pairs work on pairs of user tiles: an odd chunk gets one padding tile
     L.chunk_rows = L.chunk_ut * TM;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t at = o; o += (bytes + 1023) / 1024 * 1024; return at; };
@@ -1409,7 +1217,7 @@ static Layout make_layout(int64_t n_q, int64_t n_items, int k)
     L.off_upack = take((size_t)L.chunk_ut * TM * L.kp * 2);
     L.off_unorm = take((size_t)L.chunk_rows * 4);
     L.off_uabs = take((size_t)L.chunk_rows * 4);
-    L.off_lists = take((size_t)L.chunk_ut * 8 * CAP * 32 * 8);          // = 4 ST warps x 32 lanes x cap_for(ST) x (score + id), ST = 2 and 4
+    L.off_lists = take((size_t)L.chunk_ut * EPI_WARPS * CAP * 32 * 8);  // = EPI_WARPS x 32 lanes x CAP x (score + id)
     L.off_cnt = take((size_t)L.chunk_rows * MAX_ST * 4);
     L.off_flag = take((size_t)L.chunk_rows * MAX_ST * 4);
     L.off_tau = take((size_t)L.chunk_rows * MAX_ST * 4);
@@ -1420,82 +1228,29 @@ static Layout make_layout(int64_t n_q, int64_t n_items, int k)
     return L;
 }
 
-static size_t smem_bytes_for(int kp, int st, int cg)
+static size_t smem_bytes_for(int kp)
 {
-    const int NS = num_stages(kp, st, cg);
-    return (size_t)TM * kp * 2 + (size_t)NS * ((TN / cg) * kp * 2) + 32 * 8 + (size_t)st * TM * 8 + (size_t)st * TM * 4 * 4
-           + (size_t)st * NB * TM * 2 + 1024;
+    return (size_t)TM * kp * 2 + (size_t)num_stages(kp) * SN * kp * 2 + SMEM_FIXED;
 }
 
-// CTAs that share one MMA: 2 = CTA pairs (cta_group::2, the default), 1 = every CTA alone (B200_RANK_CTA=1, for A/B runs)
-static int rank_cta_group()
-{
-    if (const char* e = getenv("B200_RANK_CTA")) {
-        if (e[0] == '1') return 1;
-        if (e[0] == '2') return 2;
-    }
-    return 2;
-}
-
-template <bool DUMP, int ST, int CG, bool DBG = false>
+template <bool DUMP, bool DBG = false>
 static int launch_rank_tc_t(const RankTcParams& p, cudaStream_t st)
 {
-    auto kern = rank_tc_kernel<DUMP, ST, CG, DBG>;
-    const size_t smem = smem_bytes_for(p.kp, ST, CG);
+    auto kern = rank_tc_kernel<DUMP, DBG>;
+    const size_t smem = smem_bytes_for(p.kp);
     B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(threads_for(ST), 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr;
-    int max_groups = sm_count();
-    if (CG == 2) {
-        attr.id = cudaLaunchAttributeClusterDimension;
-        attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-        cfg.attrs = &attr;
-        cfg.numAttrs = 1;
-        cfg.gridDim = dim3((unsigned)(sm_count() & ~1), 1, 1);
-        int n_clusters = 0;
-        B200_CUDA(cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg));
-        B200_REQUIRE(n_clusters >= 1, "rank_tc: no CTA pair fits the device (cudaOccupancyMaxActiveClusters = %d)", n_clusters);
-        max_groups = n_clusters;
-    }
-    const int want = (p.n_ut + CG - 1) / CG;
-    const int groups = want < max_groups ? want : max_groups;
-    cfg.gridDim = dim3((unsigned)(groups * CG), 1, 1);
+    const int grid = p.n_ut < sm_count() ? p.n_ut : sm_count();
     ::b200::count_launch();
-    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
+    kern<<<grid, THREADS, smem, st>>>(p);
+    B200_CUDA(cudaGetLastError());
     return B200_OK;
 }
 
 template <bool DUMP>
-static int launch_rank_tc(const RankTcParams& p, int strips, cudaStream_t st)
+static int launch_rank_tc(const RankTcParams& p, cudaStream_t st)
 {
-    const int cg = rank_cta_group();
-    if (DUMP) return cg == 2 ? launch_rank_tc_t<DUMP, 2, 2>(p, st) : launch_rank_tc_t<DUMP, 2, 1>(p, st);
-    if (!DUMP && p.debug != 0) {             // timing experiments: the instantiation that carries the switches
-        if (strips == 4) return cg == 2 ? launch_rank_tc_t<false, 4, 2, true>(p, st) : launch_rank_tc_t<false, 4, 1, true>(p, st);
-        return cg == 2 ? launch_rank_tc_t<false, 2, 2, true>(p, st) : launch_rank_tc_t<false, 2, 1, true>(p, st);
-    }
-    if (strips == 4) return cg == 2 ? launch_rank_tc_t<DUMP, 4, 2>(p, st) : launch_rank_tc_t<DUMP, 4, 1>(p, st);
-    return cg == 2 ? launch_rank_tc_t<DUMP, 2, 2>(p, st) : launch_rank_tc_t<DUMP, 2, 1>(p, st);
-}
-
-// column strips per row (epilogue warps = 4 x strips): B200_RANK_STRIPS = 2 | 4
-static int rank_strips(int k, int topk)
-{
-    if (topk > 128) return 2;                   // 4-strip lists hold 512 entries: too close to 2 x topk
-    if (const char* e = getenv("B200_RANK_STRIPS")) {
-        if (e[0] == '4') return 4;
-        if (e[0] == '2') return 2;
-    }
-    // 64-column strips (16 epilogue warps): a warp holds its whole strip in registers, so the accumulator is handed back before
-    // any screening: 17.1 vs 14.4 M users/s at 100 K items, k = 64.  At k = 128 / 1 M items 128-column strips (8 warps, 168
-    // registers, no spills) are 3 % faster (5.63 vs 5.82 ms per 18 944 users, profiles/r02_rank_tc.md), but that variant's parity
-    // tests last ran BEFORE the batched list scans and the split of the debug branches (the round's GPU budget ended), so it
-    // stays opt-in (B200_RANK_STRIPS=2) until `pytest -m gpu` has run with it.
-    (void)k;
-    return 4;
+    if (!DUMP && p.debug != 0) return launch_rank_tc_t<false, true>(p, st);     // timing experiments: the instantiation that carries the switches
+    return launch_rank_tc_t<DUMP>(p, st);
 }
 
 }  // namespace tc
@@ -1579,7 +1334,6 @@ int rank_tc(const float* U, const int64_t* user_idx, int64_t n_q, const float* V
     uint8_t* ws = static_cast<uint8_t*>(workspace);
     // the packed item side: the caller's (built once by b200_rank_pack_items) or this call's own, in the workspace
     const uint8_t* items = packed_items ? static_cast<const uint8_t*>(packed_items) : ws;
-    const int strips = rank_strips(k, topk);
     int rc = packed_items ? B200_OK : pack_items(V, n_items, k, item_base, L, ws, st);
     if (rc) return rc;
     for (int64_t q0 = 0; q0 < n_q; q0 += L.chunk_rows) {
@@ -1587,7 +1341,7 @@ int rank_tc(const float* U, const int64_t* user_idx, int64_t n_q, const float* V
         const int64_t n_ut = (rows + TM - 1) / TM;
         const int64_t* uidx = user_idx ? user_idx + q0 : nullptr;
         const float* Usrc = user_idx ? U : U + (size_t)q0 * k;
-        rc = pack_users(Usrc, uidx, rows, (n_ut + 1) & ~(int64_t)1, k, L, ws, items, st);      // padded to a whole tile pair
+        rc = pack_users(Usrc, uidx, rows, n_ut, k, L, ws, items, st);
         if (rc) return rc;
         B200_CUDA(cudaMemsetAsync(ws + L.off_over, 0, 4, st));
         RankTcParams p;
@@ -1604,7 +1358,7 @@ int rank_tc(const float* U, const int64_t* user_idx, int64_t n_q, const float* V
         p.row_tau = reinterpret_cast<float*>(ws + L.off_tau);
         p.dump = nullptr;
         { const char* d = getenv("B200_RANK_DEBUG"); p.debug = d ? atoi(d) : 0; }
-        rc = launch_rank_tc<false>(p, strips, st);
+        rc = launch_rank_tc<false>(p, st);
         if (rc) return rc;
         FinishParams f;
         f.U = U; f.user_idx = uidx; f.q0 = q0; f.V = V; f.item_base = item_base; f.user_off = user_off;
@@ -1613,7 +1367,7 @@ int rank_tc(const float* U, const int64_t* user_idx, int64_t n_q, const float* V
         f.excl_indptr = p.excl_indptr; f.excl_indices = p.excl_indices;
         f.out_ids = out_ids + (size_t)q0 * topk; f.out_scores = out_scores + (size_t)q0 * topk;
         f.overflow_rows = reinterpret_cast<int*>(ws + L.off_over);
-        f.strips = strips; f.cap = cap_for(strips);
+        f.strips = ST; f.cap = CAP;
         f.big_rows = reinterpret_cast<int*>(ws + L.off_big);
         f.row_list = nullptr;
         const bool staged = (k % 4 == 0) && k <= 128 && ((reinterpret_cast<uintptr_t>(V) & 15) == 0);
@@ -1654,7 +1408,7 @@ int rank_tc(const float* U, const int64_t* user_idx, int64_t n_q, const float* V
         // Many overflowed rows = a degenerate score distribution (a diverged model: inf / NaN factors; thousands of exact ties):
         // row-by-row repair would cost a host round trip per user.  Redo the whole chunk on the exact path instead, in slabs
         // of score rows cut from the (now idle) candidate-list area -- same ids and scores, bounded time.
-        const int64_t list_bytes = (int64_t)L.chunk_ut * 8 * CAP * 32 * 8;
+        const int64_t list_bytes = (int64_t)L.chunk_ut * EPI_WARPS * CAP * 32 * 8;
         const int64_t slab_rows = list_bytes / (n_items * (int64_t)sizeof(float));
         if (n_over > 256 && slab_rows >= 8) {
             float* slab = reinterpret_cast<float*>(ws + L.off_lists);
@@ -1712,7 +1466,7 @@ extern "C" int b200_rank_tc_debug_scores(const float* U, int64_t n_q, const floa
     uint8_t* ws = static_cast<uint8_t*>(workspace);
     int rc = pack_items(V, n_items, k, item_base, L, ws, st);
     if (rc) return rc;
-    rc = pack_users(U, nullptr, n_q, (n_ut + 1) & ~(int64_t)1, k, L, ws, ws, st);
+    rc = pack_users(U, nullptr, n_q, n_ut, k, L, ws, ws, st);
     if (rc) return rc;
     RankTcParams p;
     p.Upack = ws + L.off_upack; p.Vpack = ws + L.off_vpack;
@@ -1727,5 +1481,5 @@ extern "C" int b200_rank_tc_debug_scores(const float* U, int64_t n_q, const floa
     p.row_tau = reinterpret_cast<float*>(ws + L.off_tau);
     p.dump = out;
     p.debug = 0;
-    return launch_rank_tc<true>(p, 2, st);
+    return launch_rank_tc<true>(p, st);
 }

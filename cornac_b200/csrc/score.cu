@@ -1,4 +1,4 @@
-// Exact scores and exact top-k for sm_100a (the reproducible reference path of the rank
+// Exact scores and exact top-k for sm_90a (the reproducible reference path of the rank
 // side; the tensor-core fused kernel in rank_fused.cu is checked against these).
 //
 // Replaces fast_dot (reference: cornac/utils/fast_dot.pyx:40-43) as used by BPR.score

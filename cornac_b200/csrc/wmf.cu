@@ -1,4 +1,4 @@
-// Weighted matrix factorisation (Hu / Koren / Volinsky, Pan et al.) training step for sm_100a.
+// Weighted matrix factorisation (Hu / Koren / Volinsky, Pan et al.) training step for sm_90a.
 //
 // Replaces one `sess.run([model.opt, model.loss])` of the reference's TensorFlow-1 graph
 //     cornac/models/wmf/wmf.py:34-55          (loss, gradients, clip to [-5, 5], AdamOptimizer)

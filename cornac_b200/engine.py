@@ -17,7 +17,7 @@ from ._lib import B200Error, check, current_stream, ptr
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise B200Error("cornac_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise B200Error("cornac_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     return _lib.load()
 
 
@@ -90,16 +90,19 @@ class BprData:
 
 
 def bpr_epoch(data, n_neg, U, V, B, lr, reg, use_bias, seed, epoch, stats, n_samples=None,
-              sample_base=0, atomic=True, exact_exp=False, unbounded=False, neg_weighted=False, hinge=False, blocked=False):
+              sample_base=0, atomic=True, exact_exp=False, unbounded=False, neg_weighted=False, hinge=False, blocked=False,
+              deterministic=False):
     """One Hogwild BPR epoch on the current stream; `stats` (int64[2] CUDA) accumulates
-    (correct, skipped)."""
+    (correct, skipped).  deterministic=True: rounds of samples that read the factors as the previous round left them,
+    their updates summed exactly -- the result repeats bit for bit from run to run."""
     L = require_cuda()
     k = U.shape[1]
     _dev(U, torch.float32, "U"), _dev(V, torch.float32, "V"), _dev(B, torch.float32, "B")
     _dev(stats, torch.int64, "stats")
     flags = ((_lib.SGD_ATOMIC if atomic else 0) | (_lib.SGD_EXACT_EXP if exact_exp else 0)
              | (_lib.SGD_UNBOUNDED if unbounded else 0) | (_lib.BPR_NEG_WEIGHTED if neg_weighted else 0)
-             | (_lib.BPR_LOSS_HINGE if hinge else 0) | (_lib.BPR_BLOCKED if blocked else 0))
+             | (_lib.BPR_LOSS_HINGE if hinge else 0) | (_lib.BPR_BLOCKED if blocked else 0)
+             | (_lib.BPR_DETERMINISTIC if deterministic else 0))
     n = data.nnz if n_samples is None else int(n_samples)
     data.prepare()
     check(L.b200_bpr_epoch(ptr(data.pairs), ptr(data.table), data.table.numel(), data.nnz, data.n_users, int(n_neg), n,
@@ -142,7 +145,7 @@ def bpr_epoch_replay(data, i_index, j_id, U, V, B, lr, reg, use_bias, stats, hin
 
 def bpr_train_host(indptr, indices, n_neg, U, V, B, lr, reg, use_bias, max_iter, key=0, replay_seeds=None,
                    atomic=True, on_epoch=None, keep_device=False, replica_sync=False, weighted_seed=None,
-                   neg_weighted=False, hinge=False, blocked=True):
+                   neg_weighted=False, hinge=False, blocked=True, deterministic=False):
     """Host-buffer entry of BPR training (what BPR.fit calls): uploads the CSR matrix and the
     factors, runs `max_iter` epochs, writes the trained factors back INTO the given numpy
     arrays U, V, B (pinned staging both ways).
@@ -216,7 +219,7 @@ def bpr_train_host(indptr, indices, n_neg, U, V, B, lr, reg, use_bias, max_iter,
         for epoch in range(max_iter):
             stats.zero_()
             bpr_epoch(data, n_neg, dU, dV, dB, lr, reg, use_bias, key, epoch, stats, atomic=atomic,
-                      neg_weighted=neg_weighted, hinge=hinge, blocked=blocked)
+                      neg_weighted=neg_weighted, hinge=hinge, blocked=blocked, deterministic=deterministic)
             if sync is not None:
                 sync.exchange()
             if on_epoch:

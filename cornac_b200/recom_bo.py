@@ -1,4 +1,4 @@
-"""Bias-only rating model on B200: drop-in for cornac.models.BaselineOnly.
+"""Bias-only rating model on an H100: drop-in for cornac.models.BaselineOnly.
 
 Same constructor arguments and behaviour as the reference class
 (cornac/models/baseline_only/recom_bo.pyx:34-214).  Its `_fit_sgd` (:101-140) is the MF loop of

@@ -1,8 +1,8 @@
-"""BPR on B200: drop-in for cornac.models.BPR.
+"""BPR on an H100: drop-in for cornac.models.BPR.
 
 Same constructor arguments, attributes and fit()/score()/rank() behaviour as the
 reference class (cornac/models/bpr/recom_bpr.pyx:65-333); the Cython/OpenMP `_fit_sgd`
-(:208-269) is replaced by the sm_100a kernels behind include/b200cornac.h.
+(:208-269) is replaced by the sm_90a kernels behind include/b200cornac.h.
 
 Modes (chosen like the reference chooses its thread count, recom_bpr.pyx:132-137):
   * seed given  -> deterministic: the mt19937 sample streams of RNGVector are reproduced on
@@ -38,7 +38,7 @@ def check_factor_width(k):
     8 slots of 32 lanes: k <= 1024 when k % 4 == 0, else k <= 256 (b200_bpr_epoch / b200_mf_epoch)."""
     k = int(k)
     if k < 1 or k > 1024 or (k % 4 != 0 and k > 256):
-        raise ValueError("k=%d is not supported: the B200 kernels take 1 <= k <= 1024 with k %% 4 == 0, or k <= 256 otherwise "
+        raise ValueError("k=%d is not supported: the GPU kernels take 1 <= k <= 1024 with k %% 4 == 0, or k <= 256 otherwise "
                          "(pad k to a multiple of 4)" % k)
     return k
 
@@ -54,7 +54,7 @@ def replay_hint(nnz, name):
 
 
 class BPR(DeviceScoringMixin, Recommender, ANNMixin):
-    """Bayesian Personalized Ranking trained and served on a B200.
+    """Bayesian Personalized Ranking trained and served on an H100.
 
     NOTE on `seed`: like the reference (which drops to ONE thread when a seed is given, recom_bpr.pyx:132-133), a seeded
     model trains in the deterministic replay mode -- reference-identical but serial-equivalent (~1e7 samples/s).  For
@@ -63,8 +63,8 @@ class BPR(DeviceScoringMixin, Recommender, ANNMixin):
 
     Parameters are those of cornac.models.BPR (k, max_iter, learning_rate, lambda_reg,
     use_bias, num_threads, trainable, verbose, init_params, seed) plus `mode` and
-    `atomic_updates` (default True: scatter with red.global.add -- no lost updates and ~3x faster on
-    B200; False = the reference's racy plain stores) in Hogwild mode.
+    `atomic_updates` (default True: scatter with red.global.add -- no lost updates;
+    False = the reference's racy plain stores) in Hogwild mode.
     `num_threads` is accepted for API compatibility and ignored (the GPU is the pool).
     """
     _b200_hinge = False          # MMMF switches the loop body to the hinge variant

@@ -1,4 +1,4 @@
-"""VEBPR and SBPR on B200: drop-ins for cornac.models.VEBPR / cornac.models.SBPR (SURVEY.md 8(f)-3).
+"""VEBPR and SBPR on an H100: drop-ins for cornac.models.VEBPR / cornac.models.SBPR (SURVEY.md 8(f)-3).
 
 Both are BPR with a THIRD item per sample -- a viewed-but-not-purchased item (VEBPR,
 cornac/models/bpr/recom_vebpr.pyx:50-392) or an item a friend has (SBPR, cornac/models/sbpr/recom_sbpr.pyx:38-300) --
@@ -28,7 +28,7 @@ def check_tri_factor_width(k):
 
 
 class VEBPR(DeviceScoringMixin, Recommender, ANNMixin):
-    """View-Enhanced BPR trained and served on a B200.  Parameters are those of cornac.models.VEBPR (k, max_iter,
+    """View-Enhanced BPR trained and served on an H100.  Parameters are those of cornac.models.VEBPR (k, max_iter,
     learning_rate, lambda_reg, num_threads, trainable, verbose, init_params, seed, alpha) plus `mode`; the train set must be a
     cornac.data.PurchaseViewDataset (its `view_matrix` = viewed-but-not-purchased CSR with sorted rows)."""
 
@@ -151,7 +151,7 @@ def prepare_social_data(X, Y):
 
 
 class SBPR(BPR):
-    """Social BPR trained and served on a B200.  Parameters are those of cornac.models.SBPR (k, max_iter, learning_rate,
+    """Social BPR trained and served on an H100.  Parameters are those of cornac.models.SBPR (k, max_iter, learning_rate,
     lambda_u, lambda_v, lambda_b, use_bias, num_threads, trainable, verbose, init_params, seed) plus `mode`; the train set
     must carry a `user_graph` modality.
 

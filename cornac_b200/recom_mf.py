@@ -1,4 +1,4 @@
-"""Biased matrix factorisation on B200: drop-in for cornac.models.MF (backend "cpu").
+"""Biased matrix factorisation on an H100: drop-in for cornac.models.MF (backend "cpu").
 
 Same constructor arguments and behaviour as the reference class
 (cornac/models/mf/recom_mf.py:31-326); `backend_cpu.fit_sgd`

@@ -1,4 +1,4 @@
-"""Weighted matrix factorisation on B200: drop-in for cornac.models.WMF.
+"""Weighted matrix factorisation on an H100: drop-in for cornac.models.WMF.
 
 Same constructor arguments, attributes (`U`, `V`) and fit()/score()/rank() behaviour as the reference class
 (cornac/models/wmf/recom_wmf.py:28-251).  The reference trains through a TensorFlow-1 graph

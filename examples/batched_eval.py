@@ -1,4 +1,4 @@
-"""Batched, device-side evaluation and recommendation with the B200 plug-ins (needs a GPU + the cornac package).
+"""Batched, device-side evaluation and recommendation with the GPU plug-ins (needs a GPU + the cornac package).
 
     python examples/batched_eval.py
 
@@ -16,7 +16,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "examples"))
-ref = os.path.join(ROOT, "baseline", "_ref")
+ref = os.path.join(ROOT, "oracle", "_ref")
 if os.path.isdir(os.path.join(ref, "cornac")):
     sys.path.insert(0, ref)
 

@@ -1,4 +1,4 @@
-"""cornac.Experiment with the B200 plug-ins next to the reference models (needs a GPU + the cornac package).
+"""cornac.Experiment with the GPU plug-ins next to the reference models (needs a GPU + the cornac package).
 
     python examples/bpr_experiment.py
 
@@ -13,7 +13,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-ref = os.path.join(ROOT, "baseline", "_ref")
+ref = os.path.join(ROOT, "oracle", "_ref")
 if os.path.isdir(os.path.join(ref, "cornac")):
     sys.path.insert(0, ref)
 
@@ -46,16 +46,16 @@ def ml100k_like(seed=123):
 
 
 if __name__ == "__main__":
-    # CUDA context + library load happen here, not inside the first B200 model's fit(): Train (s) then compares training
+    # CUDA context + library load happen here, not inside the first GPU model's fit(): Train (s) then compares training
     cornac_b200.engine.warmup()
     rs = RatioSplit(data=ml100k_like(), test_size=0.2, rating_threshold=4.0, exclude_unknowns=True, seed=123, verbose=True)
     models = [
         cornac.models.BPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, seed=123, name="BPR (reference, seeded)"),
-        cornac_b200.BPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, seed=123, name="BPR (B200, seeded replay)"),
-        cornac_b200.BPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, name="BPR (B200, Hogwild)"),
-        cornac_b200.WBPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, name="WBPR (B200, Hogwild)"),
+        cornac_b200.BPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, seed=123, name="BPR (GPU, seeded replay)"),
+        cornac_b200.BPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, name="BPR (GPU, Hogwild)"),
+        cornac_b200.WBPR(k=10, max_iter=200, learning_rate=0.001, lambda_reg=0.01, name="WBPR (GPU, Hogwild)"),
         cornac.models.MF(k=10, max_iter=25, learning_rate=0.01, lambda_reg=0.02, use_bias=True, seed=123, name="MF (reference, seeded)"),
-        cornac_b200.MF(k=10, max_iter=25, learning_rate=0.01, lambda_reg=0.02, use_bias=True, seed=123, name="MF (B200, ordered)"),
+        cornac_b200.MF(k=10, max_iter=25, learning_rate=0.01, lambda_reg=0.02, use_bias=True, seed=123, name="MF (GPU, ordered)"),
     ]
     metrics = [AUC(), MAP(), NDCG(k=10), Precision(k=10), Recall(k=10)]
     cornac.Experiment(eval_method=rs, models=models, metrics=metrics, user_based=True).run()

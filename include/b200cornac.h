@@ -1,5 +1,5 @@
 /*
- * b200cornac.h -- C ABI of libb200cornac.so: the B200 (sm_100a) implementation of
+ * b200cornac.h -- C ABI of libb200cornac.so: the H100 (sm_90a) implementation of
  * Cornac's embedding train-and-rank hot path (BPR / MF SGD, per-user score + rank).
  *
  * The reference has no C ABI for this path: its kernels are Cython `def`/`cpdef`
@@ -45,6 +45,9 @@ extern "C" {
 #define B200_BPR_NEG_WEIGHTED 8u /* WBPR (recom_wbpr.pyx:125-136): j = item of a uniformly drawn INTERACTION */
 #define B200_BPR_LOSS_HINGE 16u  /* MMMF (cornac/models/mmmf/recom_mmmf.pyx:129-154): hinge loss, biases always trained */
 #define B200_SGD_UNBOUNDED 4u /* do not cap the number of concurrently running samples (see b200_bpr_epoch) */
+#define B200_BPR_DETERMINISTIC 64u /* rounds of at most 16384 samples that read the factors as the previous round left them;
+                                   * a round's updates are summed exactly (fixed point) and applied once: the epoch's result
+                                   * depends on the arguments only, not on thread timing (B200_SGD_ATOMIC is then implied) */
 #define B200_BPR_BLOCKED 32u /* cache-blocked sample ORDER (same per-epoch law, see b200_bpr_block_plan): the epoch visits the
                               * interaction list window by window and the items block by block so that the rows in use stay in
                               * the L2; a no-op for matrices whose factors already fit (plan 1 x 1) */
@@ -79,7 +82,7 @@ B200_API int b200_bpr_prepare(const int32_t* indptr, const int32_t* indices, int
  * (sample_base + s, epoch)), skipping (not redrawing) a sample when user u already has
  * item j (recom_bpr.pyx:241-243), otherwise applying the update of recom_bpr.pyx:249-267
  * to U[u], V[i], V[j], B[i], B[j].  Updates are scattered with red.global.add (B200_SGD_ATOMIC,
- * no lost updates; recommended and ~3x faster on B200) or plain stores (the reference's racy
+ * no lost updates; recommended) or plain stores (the reference's racy
  * Hogwild).  At most min(n_users, n_neg)/4 samples run concurrently so that small matrices
  * are not trained from hopelessly stale rows (B200_SGD_UNBOUNDED lifts the cap).
  *   U device f32[*, k], V device f32[*, k], B device f32[*]
@@ -250,7 +253,7 @@ B200_API int b200_topk_rows(const float* scores, int64_t n_q, int64_t n_items,
 
 /* Fused rank: scores (as b200_score_batch) + exclusion + top-k (as b200_topk_rows) for a
  * batch of users without materialising the [n_q, n_items] score matrix.  Tensor-core
- * (tcgen05) candidate pass + exact f64 re-score of the candidates; ids and scores are
+ * (wgmma) candidate pass + exact f64 re-score of the candidates; ids and scores are
  * identical to b200_score_batch followed by b200_topk_rows.
  *   workspace: device scratch of b200_rank_topk_workspace_bytes(...) bytes.                */
 B200_API int64_t b200_rank_topk_workspace_bytes(int64_t n_q, int64_t n_items, int k, int topk);

@@ -7,15 +7,15 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 if os.path.isdir(os.path.join(REF, "cornac")) and REF not in sys.path:
-    sys.path.insert(0, REF)          # the unmodified reference install (git-ignored, travels with gpurun)
+    sys.path.insert(0, REF)          # the unmodified reference install (git-ignored, built by oracle/build_ref.sh)
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def golden(name):
@@ -30,7 +30,7 @@ def have_cornac():
         return False
 
 
-needs_cornac = pytest.mark.skipif(not have_cornac(), reason="reference cornac install (baseline/_ref) not importable")
+needs_cornac = pytest.mark.skipif(not have_cornac(), reason="reference cornac install (oracle/_ref) not importable")
 
 
 def rel_err(a, b):

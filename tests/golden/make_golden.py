@@ -1,7 +1,7 @@
 """Generate the committed golden vectors from the UNMODIFIED compiled reference.
 
-TEST INFRASTRUCTURE.  Run in the build container (needs baseline/_ref, i.e.
-`bash baseline/build_ref.sh` first):
+TEST INFRASTRUCTURE.  Run in the build container (needs oracle/_ref, i.e.
+`bash oracle/build_ref.sh` first):
 
     python tests/golden/make_golden.py
 
@@ -19,7 +19,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-sys.path.insert(0, os.path.join(ROOT, "baseline", "_ref"))
+sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
 
 import cornac  # noqa: E402
 from cornac.data import Dataset  # noqa: E402

@@ -425,3 +425,86 @@ def test_windowed_replay_is_bit_identical_to_serial_replay(hot, monkeypatch):
     Ur, Vr, Br = U0.copy(), V0.copy(), B0.copy()
     c_ref, s_ref = O.bpr_replay(ii, jj, indptr, indices, Ur, Vr, Br, 0.05, 0.01, True)
     assert outs[1][3][1] == s_ref and rel_err(outs[1][0], Ur) < 1e-5 and rel_err(outs[1][1], Vr) < 1e-5
+
+
+@pytest.mark.parametrize("k", [10, 128])
+def test_deterministic_epoch_repeats_bit_for_bit_and_trains(k):
+    """deterministic=True (what fit() and the bench run): two runs of the same blocked epochs give identical factors and
+    counts; the skip count equals the oracle's on the same stream; with lr = 0 the factors are untouched; the model
+    learns (more correctly ranked samples in the last epoch than in the first)."""
+    import torch
+    from cornac_b200 import engine
+    n_users, n_items = 30000, 3000
+    indptr, indices = synth_csr(n_users, n_items, 600000, seed=8)
+    nnz = len(indices)
+    rng = np.random.RandomState(2)
+    U0 = rng.normal(0, 0.1, (n_users, k)).astype(np.float32)
+    V0 = rng.normal(0, 0.1, (n_items, k)).astype(np.float32)
+    B0 = np.zeros(n_items, np.float32)
+    data = _data(indptr, indices)
+    runs = []
+    for _ in range(2):
+        U, V, B = _dev(U0), _dev(V0), _dev(B0)
+        counts = []
+        for e in range(4):
+            stats = torch.zeros(2, dtype=torch.int64, device="cuda")
+            engine.bpr_epoch(data, n_items, U, V, B, 0.05, 0.01, True, 31, e, stats, blocked=True, deterministic=True)
+            counts.append(tuple(stats.cpu().tolist()))
+        runs.append((U.cpu().numpy(), V.cpu().numpy(), B.cpu().numpy(), counts))
+    for a, b in zip(runs[0][:3], runs[1][:3]):
+        assert np.array_equal(a, b)
+    assert runs[0][3] == runs[1][3]
+    assert runs[0][3][-1][0] > runs[0][3][0][0]
+    U, V, B = _dev(U0), _dev(V0), _dev(B0)
+    stats = torch.zeros(2, dtype=torch.int64, device="cuda")
+    engine.bpr_epoch(data, n_items, U, V, B, 0.0, 0.01, True, 31, 0, stats, deterministic=True, exact_exp=True)
+    assert np.array_equal(U.cpu().numpy(), U0) and np.array_equal(V.cpu().numpy(), V0)
+    ii, jj = engine.bpr_draw_host(31, 0, nnz, nnz, n_items)
+    c_ref, s_ref = O.bpr_replay(ii, jj, indptr, indices, U0.copy(), V0.copy(), B0.copy(), 0.0, 0.01, True)
+    c, s = stats.cpu().tolist()
+    assert s == s_ref and abs(c - c_ref) <= 3
+
+
+@pytest.mark.parametrize("k", [10, 64])
+def test_deterministic_round_equals_numpy_restatement(k):
+    """ONE round of the deterministic mode (16384 samples, unbounded): every live sample's update is computed from the
+    factors as they were at the start of the round and the updates are summed -- restated here in float64 with numpy,
+    sample by sample from the host copy of the Philox stream; the changes of U, V and B and the counts must agree."""
+    import torch
+    from cornac_b200 import engine
+    n_users, n_items, n = 30000, 3000, 16384
+    indptr, indices = synth_csr(n_users, n_items, 600000, seed=9)
+    nnz = len(indices)
+    rng = np.random.RandomState(3)
+    U0 = rng.normal(0, 0.1, (n_users, k)).astype(np.float32)
+    V0 = rng.normal(0, 0.1, (n_items, k)).astype(np.float32)
+    B0 = rng.normal(0, 0.1, n_items).astype(np.float32)
+    lr, reg = 0.05, 0.01
+    data = _data(indptr, indices)
+    U, V, B = _dev(U0), _dev(V0), _dev(B0)
+    stats = torch.zeros(2, dtype=torch.int64, device="cuda")
+    engine.bpr_epoch(data, n_items, U, V, B, lr, reg, True, 5, 3, stats, n_samples=n, exact_exp=True, unbounded=True,
+                     deterministic=True)
+    ii, jj = engine.bpr_draw_host(5, 3, n, nnz, n_items)
+    users = np.repeat(np.arange(n_users), np.diff(indptr))[ii]
+    pos = indices[ii]
+    dU, dV, dB = np.zeros(U0.shape), np.zeros(V0.shape), np.zeros(B0.shape)
+    correct = skipped = 0
+    U64, V64, B64 = U0.astype(np.float64), V0.astype(np.float64), B0.astype(np.float64)
+    for u, i, j in zip(users, pos, jj):
+        if j in indices[indptr[u]:indptr[u + 1]]:
+            skipped += 1
+            continue
+        score = B64[i] - B64[j] + U64[u] @ (V64[i] - V64[j])
+        z = 1.0 / (1.0 + np.exp(score))
+        correct += z < 0.5
+        dU[u] += lr * (z * (V64[i] - V64[j]) - reg * U64[u])
+        dV[i] += lr * (z * U64[u] - reg * V64[i])
+        dV[j] += lr * (-z * U64[u] - reg * V64[j])
+        dB[i] += lr * (z - reg * B64[i])
+        dB[j] += lr * (-z - reg * B64[j])
+    c, s = stats.cpu().tolist()
+    assert s == skipped and abs(c - correct) <= 3
+    assert rel_err(U.cpu().numpy().astype(np.float64) - U64, dU) < 1e-4
+    assert rel_err(V.cpu().numpy().astype(np.float64) - V64, dV) < 1e-4
+    assert rel_err(B.cpu().numpy().astype(np.float64) - B64, dB) < 1e-4

@@ -1,5 +1,5 @@
 """The drop-in plug-ins through the reference's own Python stack (unchanged cornac from
-baseline/_ref): fit / score / rank / ranking_eval / Experiment / clone / save-load.  GPU only.
+oracle/_ref): fit / score / rank / ranking_eval / Experiment / clone / save-load.  GPU only.
 Mirrors the reference's smoke tests (tests/cornac/models/test_recommender.py:28-53,
 tests/cornac/eval_methods/test_ratio_split.py:92-109, tests/cornac/test_hyperopt.py:39-55)
 and adds the value checks the reference lacks."""

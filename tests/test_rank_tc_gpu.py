@@ -1,4 +1,4 @@
-"""Tensor-core (tcgen05) rank path: the approximate pass against an fp16 matmul, and the fused
+"""Tensor-core (wgmma) rank path: the approximate pass against an fp16 matmul, and the fused
 b200_rank_topk against the oracle -- ids and scores bit-exact.  GPU only."""
 import os
 
@@ -41,7 +41,7 @@ def _rank_topk(U, V, base, uidx, uoff, excl, topk):
 
 @pytest.mark.parametrize("k,n_items,n_q", [(16, 1024, 128), (64, 1500, 100), (128, 3000, 260), (100, 2048, 37), (8, 1100, 5)])
 def test_tensor_pass_matches_fp16_matmul(k, n_items, n_q):
-    """UMMA descriptors / packing / power-of-two scaling / TMEM read-back: dense approximate scores ==
+    """GMMA descriptors / packing / power-of-two scaling / accumulator hand-off: dense approximate scores ==
     fp16 x fp16 -> f32 of the scaled operands, unscaled."""
     import torch
     from cornac_b200._lib import check, current_stream, load, ptr
@@ -220,25 +220,3 @@ def test_packed_item_side_built_once_gives_the_same_answer_and_is_really_used():
     assert engine.rank_pack_items(torch.zeros((500, 64), device="cuda")) is None      # tiny catalogue: exact path, nothing to pack
     with pytest.raises(Exception):
         engine.rank_topk(U, V[:4000].contiguous(), 20, packed_items=packed)
-
-
-@pytest.mark.parametrize("n_q", [1, 129, 300, 1000])
-def test_cta_pair_kernel_equals_single_cta_kernel(monkeypatch, n_q):
-    """cta_group::2 (two CTAs of a cluster share one M = 256 MMA, each staging half of every V tile; the default) and the
-    single-CTA kernel (B200_RANK_CTA=1) nominate candidates independently; after the exact finish both give the oracle's
-    ids and scores -- odd tile counts (a padding tile in the last pair), one tile, many tiles per pair."""
-    rng = np.random.RandomState(n_q)
-    k, n_items, topk = 64, 9000, 50
-    U = rng.normal(0, 0.3, (n_q, k)).astype(np.float32)
-    V = rng.normal(0, 0.3, (n_items, k)).astype(np.float32)
-    base = rng.normal(0, 0.3, n_items).astype(np.float32)
-    excl = [np.unique(rng.randint(n_items, size=rng.randint(0, 120))) for _ in range(n_q)]
-    monkeypatch.setenv("B200_RANK_CTA", "2")
-    a = _rank_topk(U, V, base, None, None, excl, topk)
-    monkeypatch.setenv("B200_RANK_CTA", "1")
-    b = _rank_topk(U, V, base, None, None, excl, topk)
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
-    want = O.score_batch(U, V, base)
-    for q in range(0, n_q, 7):
-        wi, ws, w = O.topk(want[q], topk, excl[q])
-        assert np.array_equal(a[0][q], wi) and np.array_equal(a[1][q][:w], ws[:w])

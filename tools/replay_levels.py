@@ -4,8 +4,7 @@ A sample (u, i, j) must see every earlier update of its three rows; samples that
 dependency level of a sample = 1 + the largest level among earlier samples that touch one of its rows; all samples of
 one level are independent, and the number of levels is the length of the critical path = the number of sequential steps
 ANY exact schedule needs.  The windowed replay kernel (bpr_replay_window_kernel) resolves this inside windows of 32
-samples; this script measures what window sizes up to the whole epoch would allow (numbers in
-profiles/r01_tune_replay.txt).  Pure numpy + the host sampler of libb200cornac.so; no GPU."""
+samples; this script measures what window sizes up to the whole epoch would allow.  Pure numpy + the host sampler of libb200cornac.so; no GPU."""
 import os
 import sys
 
