@@ -1,15 +1,15 @@
 // BPR SGD epochs for sm_90a.
 //
 // Replaces BPR._fit_sgd (reference: cornac/models/bpr/recom_bpr.pyx:208-269) with
-//   * bpr_hogwild_kernel : throughput mode.  Persistent grid; every G-lane group draws its
-//     own (u, i+, j-) triplets from the CSR matrix with a counter-based RNG, gathers the
-//     three factor rows with 128-bit L2-only loads, reduces the pairwise dot with warp
-//     shuffles and scatters the update back (plain 128-bit stores = the reference's
-//     lock-free Hogwild, or red.global.add.v4.f32 when B200_SGD_ATOMIC is set).
-//   * bpr_replay_kernel  : parity mode.  One warp applies an explicit sample stream with
-//     the same result as the sequential seeded reference (num_threads = 1,
-//     recom_bpr.pyx:132-133): sample metadata (u, i, j, skip test) is resolved 32 samples
-//     at a time in parallel (read-only data), the updates are applied strictly in order.
+//   * throughput mode (Hogwild): persistent grids in which every G-lane group draws its own (u, i+, j-) triplets from
+//     the CSR matrix with a counter-based RNG, gathers the three factor rows with L2-only loads, reduces the pairwise
+//     dot with warp shuffles and scatters the update back (plain stores = the reference's lock-free Hogwild, or
+//     red.global.add when B200_SGD_ATOMIC is set).  launch_hogwild picks one kernel per row layout:
+//     bpr_hogwild_stream_kernel, bpr_hogwild_chunk_kernel or bpr_hogwild_kernel.
+//   * deterministic mode: bpr_det_grad_kernel + bpr_det_apply_kernel, the same law and updates in fixed rounds.
+//   * parity mode: bpr_replay_sched_kernel applies an explicit sample stream with the same result as the sequential
+//     seeded reference (num_threads = 1, recom_bpr.pyx:132-133); bpr_replay_kernel (one warp, strictly serial) is the
+//     reference it is checked against.
 //
 // HBM-bound integer/gather work: no tensor cores here by design (DESIGN.md, K1).
 #include <stdlib.h>
@@ -36,6 +36,12 @@ __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x)
     return x;
 }
 
+// key of the pair (u, i) in the membership table
+__device__ __forceinline__ uint64_t pair_key(int32_t u, int32_t i)
+{
+    return ((uint64_t)(uint32_t)u << 32) | (uint32_t)i;
+}
+
 struct BprParams {
     const int2* __restrict__ pairs;
     const unsigned long long* __restrict__ table;   // 4 slots (32 B) per bucket
@@ -45,7 +51,6 @@ struct BprParams {
     int64_t n_samples;
     int64_t max_groups;          // cap on concurrently running samples (Hogwild staleness bound)
     int exact_exp;               // B200_SGD_EXACT_EXP
-    int debug_skip;              // profiling only (B200_BPR_DEBUG_SKIP): bit0 U, bit1 V+, bit2 V- scatter off
     int hinge;                   // MMMF (recom_mmmf.pyx:129-154): skip correctly ranked pairs, z = 1 otherwise
     int neg_weighted;            // WBPR: negatives drawn from the interaction list (popularity-weighted)
     SampleLaw law;               // unblocked or cache-blocked sample order (common.cuh)
@@ -68,16 +73,139 @@ __device__ __forceinline__ float bpr_z(float score, int exact)
     return __frcp_rn(1.f + __expf(score));
 }
 
-// resident blocks per SM the register allocator is asked to make room for: the kernel is
-// latency-bound on dependent gathers, so samples in flight per SM (= groups x S) is the lever
-template <int NPL, bool VEC, int S>
-constexpr int hogwild_min_blocks()
+// z of a sample and its count as correctly ranked.  MMMF (recom_mmmf.pyx:137-139) does not update a correctly ranked
+// pair (returns false) and uses z = 1 otherwise.
+template <class Count>
+__device__ __forceinline__ bool sample_z(int hinge, int exact, float score, float& z, Count& n_correct)
 {
-    constexpr int E = NPL * (VEC ? 4 : 1);
-    return (E * S <= 4) ? 5 : (E * S <= 8) ? 4 : (E * S <= 16) ? 2 : 1;
+    if (hinge) {
+        if (score > 0.f) { ++n_correct; return false; }
+        z = 1.f;
+    } else {
+        z = bpr_z(score, exact);
+        n_correct += (z < .5f);
+    }
+    return true;
 }
 
-template <int G, int NPL, bool VEC, bool ATOMIC, int S, int MINB>
+// ---------------------------------------------------------------------------------------
+// Pieces shared by the throughput kernels.
+
+// Sample s_local of the epoch (the law of common.cuh): its interaction index ii and its negative j.  A WBPR negative is
+// the item of a uniformly drawn interaction (recom_wbpr.pyx:131).  The caller gathers pairs[ii] itself, where the
+// latency of that load fits its schedule.
+__device__ __forceinline__ void draw_sample(const BprParams& p, int64_t s_local, int64_t& ii, int32_t& j)
+{
+    const uint64_t s = p.sample_base + (uint64_t)s_local;
+    const Philox4 r = philox4x32_10((uint32_t)s, (uint32_t)(s >> 32), p.epoch_lo, p.epoch_hi, p.seed_lo, p.seed_hi);
+    int64_t i_lo, i_len, j_lo, j_len;
+    law_ranges(p.law, s, i_lo, i_len, j_lo, j_len);
+    ii = i_lo + (int64_t)range64(r.x, r.y, (uint64_t)i_len);
+    j = p.neg_weighted ? __ldg(p.pairs + range64(r.z, r.w, (uint64_t)p.nnz)).y
+                       : (int32_t)(j_lo + (int64_t)range64(r.z, r.w, (uint64_t)j_len));
+}
+
+// has_non_zero(u, j) (recom_bpr.pyx:241-243) by one lane: `key` in `bucket` (two 16-byte loads) or in the buckets it
+// overflowed into
+__device__ __forceinline__ bool bucket_has(const unsigned long long* table, uint64_t mask, uint64_t key, uint64_t bucket)
+{
+    bool found, full;
+    do {
+        const ulonglong2 b0 = __ldg(reinterpret_cast<const ulonglong2*>(table + 4 * bucket));
+        const ulonglong2 b1 = __ldg(reinterpret_cast<const ulonglong2*>(table + 4 * bucket) + 1);
+        found = (b0.x == key) | (b0.y == key) | (b1.x == key) | (b1.y == key);
+        full = (b1.y != TABLE_EMPTY);
+        bucket = (bucket + 1) & mask;
+    } while (!found && full);              // rare: the bucket overflowed into the next one
+    return found;
+}
+
+// The same test by a G-lane group: lanes 0-3 read the four slots of a bucket, 8 bytes each
+template <int G>
+__device__ __forceinline__ bool group_has(const unsigned long long* table, uint64_t mask, uint64_t key, uint64_t bucket,
+                                          int lg)
+{
+    const unsigned gmask = group_mask<G>();
+    for (;;) {
+        const unsigned long long sl = (lg < 4) ? __ldg(table + 4 * bucket + lg) : 0ull;
+        const unsigned hit = __ballot_sync(gmask, lg < 4 && sl == key) & gmask;
+        const unsigned full = __ballot_sync(gmask, lg == 3 && sl != TABLE_EMPTY) & gmask;
+        if (hit) return true;
+        if (!full) return false;
+        bucket = (bucket + 1) & mask;      // rare: the bucket overflowed into the next one
+    }
+}
+
+// Block epilogue: the block's (correct, skipped) counts added to the epoch statistics with two atomics.  Every thread
+// passes its own share, so a count kept by the whole group goes in from one lane of the group only.
+__device__ __forceinline__ void flush_stats(unsigned int correct, unsigned int skipped, unsigned long long* stats)
+{
+    __shared__ unsigned int sh_stats[2];
+    if (threadIdx.x < 2) sh_stats[threadIdx.x] = 0;
+    __syncthreads();
+    correct = __reduce_add_sync(0xffffffffu, correct);
+    skipped = __reduce_add_sync(0xffffffffu, skipped);
+    if ((threadIdx.x & 31) == 0) {
+        atomicAdd(&sh_stats[0], correct);
+        atomicAdd(&sh_stats[1], skipped);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        atomicAdd(stats + 0, (unsigned long long)sh_stats[0]);
+        atomicAdd(stats + 1, (unsigned long long)sh_stats[1]);
+    }
+}
+
+// The SGD step of sample (u, i, j) from the group's fragments of its rows (recom_bpr.pyx:253-267): red.add of the
+// deltas (ATOMIC) or plain stores of the updated rows and biases
+template <int G, int NPL, bool VEC, bool ATOMIC>
+__device__ __forceinline__ void frag_update(const BprParams& p, RowFrag<NPL, VEC>& fu, RowFrag<NPL, VEC>& fi,
+                                            RowFrag<NPL, VEC>& fj, float bi, float bj, int32_t u, int32_t i, int32_t j,
+                                            float z, int lg, int n_units)
+{
+    constexpr int E = NPL * RowFrag<NPL, VEC>::W;
+    const float lr = p.lr, reg = p.reg;
+    const size_t k = (size_t)p.k;
+    float* pu = p.U + (size_t)u * k;
+    float* pi = p.V + (size_t)i * k;
+    float* pj = p.V + (size_t)j * k;
+    if (ATOMIC) {
+        RowFrag<NPL, VEC> du, di, dj;
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const float uf = fu.v[e], vi = fi.v[e], vj = fj.v[e];
+            du.v[e] = lr * (z * (vi - vj) - reg * uf);
+            di.v[e] = lr * (z * uf - reg * vi);
+            dj.v[e] = lr * (-z * uf - reg * vj);
+        }
+        row_red_add<G, NPL, VEC>(du, pu, lg, n_units);
+        row_red_add<G, NPL, VEC>(di, pi, lg, n_units);
+        row_red_add<G, NPL, VEC>(dj, pj, lg, n_units);
+        if (p.use_bias && lg == 0) {
+            red_add_f32(p.B + i, lr * (z - reg * bi));
+            red_add_f32(p.B + j, lr * (-z - reg * bj));
+        }
+    } else {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const float uf = fu.v[e], vi = fi.v[e], vj = fj.v[e];
+            fu.v[e] = uf + lr * (z * (vi - vj) - reg * uf);
+            fi.v[e] = vi + lr * (z * uf - reg * vi);
+            fj.v[e] = vj + lr * (-z * uf - reg * vj);
+        }
+        row_store<G, NPL, VEC>(fu, pu, lg, n_units);
+        row_store<G, NPL, VEC>(fi, pi, lg, n_units);
+        row_store<G, NPL, VEC>(fj, pj, lg, n_units);
+        if (p.use_bias && lg == 0) {
+            __stcg(p.B + i, bi + lr * (z - reg * bi));
+            __stcg(p.B + j, bj + lr * (-z - reg * bj));
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------
+// One sample per G-lane group, rows in registers: the layouts with 16 or 32 floats of a row per lane (k > 256).
+template <int G, int NPL, bool VEC, bool ATOMIC, int MINB>
 __global__ void __launch_bounds__(256, MINB) bpr_hogwild_kernel(const BprParams p)
 {
     using Frag = RowFrag<NPL, VEC>;
@@ -91,144 +219,47 @@ __global__ void __launch_bounds__(256, MINB) bpr_hogwild_kernel(const BprParams 
 
     unsigned int n_correct = 0, n_skipped = 0;
 
-    for (int64_t s0 = gid * S; s0 < p.n_samples; s0 += n_groups * S) {
-        int32_t u[S], it[S], jt[S];
-        bool live[S];
-        Frag fu[S], fi[S], fj[S];
-        float bi[S], bj[S];
-        // ---- phase A: draw the triplets (every lane of the group computes the same values);
-        //      the negative row does not depend on the interaction gather, so it goes out first
-        int2 pr[S];
+    for (int64_t s = gid; s < p.n_samples; s += n_groups) {
+        // ---- draw the triplet (every lane of the group computes the same values); the negative row does not depend on
+        //      the interaction gather, so it goes out first
+        int64_t ii;
+        int32_t j;
+        draw_sample(p, s, ii, j);
+        const int2 pr = __ldg(p.pairs + ii);
+        Frag fu, fi, fj;
+        row_load<G, NPL, VEC>(fj, p.V + (size_t)j * k, lg, n_units);
+        const float bj = __ldcg(p.B + j);
+        // ---- user row, positive row and the membership bucket (has_non_zero(u, j), recom_bpr.pyx:241-243), all in
+        //      flight together
+        const int32_t u = pr.x, i = pr.y;
+        row_load<G, NPL, VEC>(fu, p.U + (size_t)u * k, lg, n_units);
+        row_load<G, NPL, VEC>(fi, p.V + (size_t)i * k, lg, n_units);
+        const float bi = __ldcg(p.B + i);
+        const uint64_t key = pair_key(u, j);
+        const bool skip = group_has<G>(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask, lg);
+        n_skipped += skip;
+        // ---- score, z, update (recom_bpr.pyx:249-267)
+        float part = 0.f;
 #pragma unroll
-        for (int t = 0; t < S; ++t) {
-            const uint64_t s = p.sample_base + (uint64_t)(s0 + t);
-            live[t] = (s0 + t) < p.n_samples;
-            Philox4 r = philox4x32_10((uint32_t)s, (uint32_t)(s >> 32), p.epoch_lo, p.epoch_hi, p.seed_lo, p.seed_hi);
-            int64_t i_lo, i_len, j_lo, j_len;
-            law_ranges(p.law, s, i_lo, i_len, j_lo, j_len);
-            const int64_t ii = i_lo + (int64_t)range64(r.x, r.y, (uint64_t)i_len);
-            jt[t] = p.neg_weighted ? __ldg(p.pairs + range64(r.z, r.w, (uint64_t)p.nnz)).y
-                                   : (int32_t)(j_lo + (int64_t)range64(r.z, r.w, (uint64_t)j_len));
-            pr[t] = __ldg(p.pairs + ii);
-            row_load<G, NPL, VEC>(fj[t], p.V + (size_t)jt[t] * k, lg, n_units);
-            bj[t] = __ldcg(p.B + jt[t]);
-        }
-        // ---- phase B: user row, positive row and the membership bucket, all in flight together.
-        //      The 32-byte bucket is read by the first four lanes of the group, 8 bytes each.
-        unsigned long long slot[S];
-        uint64_t bkt[S];
-#pragma unroll
-        for (int t = 0; t < S; ++t) {
-            u[t] = pr[t].x;
-            it[t] = pr[t].y;
-            const uint64_t key = ((uint64_t)(uint32_t)u[t] << 32) | (uint32_t)jt[t];
-            bkt[t] = mix64(key) & p.bucket_mask;
-            slot[t] = (lg < 4) ? __ldg(p.table + 4 * bkt[t] + lg) : 0ull;
-            row_load<G, NPL, VEC>(fu[t], p.U + (size_t)u[t] * k, lg, n_units);
-            row_load<G, NPL, VEC>(fi[t], p.V + (size_t)it[t] * k, lg, n_units);
-            bi[t] = __ldcg(p.B + it[t]);
-        }
-        // ---- phase C: has_non_zero(u, j)  (recom_bpr.pyx:241-243) = key (u, j) in the table
-        const unsigned gmask = group_mask<G>();
-#pragma unroll
-        for (int t = 0; t < S; ++t) {
-            const uint64_t key = ((uint64_t)(uint32_t)u[t] << 32) | (uint32_t)jt[t];
-            unsigned hit = __ballot_sync(gmask, lg < 4 && slot[t] == key) & gmask;
-            unsigned full = __ballot_sync(gmask, lg == 3 && slot[t] != TABLE_EMPTY) & gmask;
-            uint64_t bb = bkt[t];
-            while (!hit && full) {            // rare: the bucket overflowed into the next one
-                bb = (bb + 1) & p.bucket_mask;
-                const unsigned long long sl = (lg < 4) ? __ldg(p.table + 4 * bb + lg) : 0ull;
-                hit = __ballot_sync(gmask, lg < 4 && sl == key) & gmask;
-                full = __ballot_sync(gmask, lg == 3 && sl != TABLE_EMPTY) & gmask;
-            }
-            if (live[t] && hit) {
-                live[t] = false;
-                ++n_skipped;
-            }
-        }
-        // ---- phase D: score, z, update (recom_bpr.pyx:249-267)
-#pragma unroll
-        for (int t = 0; t < S; ++t) {
-            float part = 0.f;
-#pragma unroll
-            for (int e = 0; e < E; ++e) part = fmaf(fu[t].v[e], fi[t].v[e] - fj[t].v[e], part);
-            const float score = (bi[t] - bj[t]) + group_sum<G>(part);
-            if (!live[t]) continue;     // group-uniform
-            float z;
-            if (p.hinge) {
-                if (score > 0.f) { ++n_correct; continue; }
-                z = 1.f;
-            } else {
-                z = bpr_z(score, p.exact_exp);
-                n_correct += (z < .5f);
-            }
-            const float lr = p.lr, reg = p.reg;
-            float* pu = p.U + (size_t)u[t] * k;
-            float* pi = p.V + (size_t)it[t] * k;
-            float* pj = p.V + (size_t)jt[t] * k;
-            if (ATOMIC) {
-                Frag du, di, dj;
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const float uf = fu[t].v[e], vi = fi[t].v[e], vj = fj[t].v[e];
-                    du.v[e] = lr * (z * (vi - vj) - reg * uf);
-                    di.v[e] = lr * (z * uf - reg * vi);
-                    dj.v[e] = lr * (-z * uf - reg * vj);
-                }
-                row_red_add<G, NPL, VEC>(du, pu, lg, n_units);
-                row_red_add<G, NPL, VEC>(di, pi, lg, n_units);
-                row_red_add<G, NPL, VEC>(dj, pj, lg, n_units);
-                if (p.use_bias && lg == 0) {
-                    red_add_f32(p.B + it[t], lr * (z - reg * bi[t]));
-                    red_add_f32(p.B + jt[t], lr * (-z - reg * bj[t]));
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const float uf = fu[t].v[e], vi = fi[t].v[e], vj = fj[t].v[e];
-                    fu[t].v[e] = uf + lr * (z * (vi - vj) - reg * uf);
-                    fi[t].v[e] = vi + lr * (z * uf - reg * vi);
-                    fj[t].v[e] = vj + lr * (-z * uf - reg * vj);
-                }
-                row_store<G, NPL, VEC>(fu[t], pu, lg, n_units);
-                row_store<G, NPL, VEC>(fi[t], pi, lg, n_units);
-                row_store<G, NPL, VEC>(fj[t], pj, lg, n_units);
-                if (p.use_bias && lg == 0) {
-                    __stcg(p.B + it[t], bi[t] + lr * (z - reg * bi[t]));
-                    __stcg(p.B + jt[t], bj[t] + lr * (-z - reg * bj[t]));
-                }
-            }
-        }
+        for (int e = 0; e < E; ++e) part = fmaf(fu.v[e], fi.v[e] - fj.v[e], part);
+        const float score = (bi - bj) + group_sum<G>(part);
+        if (skip) continue;     // group-uniform
+        float z;
+        if (!sample_z(p.hinge, p.exact_exp, score, z, n_correct)) continue;
+        frag_update<G, NPL, VEC, ATOMIC>(p, fu, fi, fj, bi, bj, u, i, j, z, lg, n_units);
     }
-
-    // ---- epoch statistics: one count per group (its lane 0), block-reduced, two atomics per block
-    __shared__ unsigned int sh_stats[2];
-    if (threadIdx.x < 2) sh_stats[threadIdx.x] = 0;
-    __syncthreads();
-    unsigned int c = (lg == 0) ? n_correct : 0u, sk = (lg == 0) ? n_skipped : 0u;
-    c = __reduce_add_sync(0xffffffffu, c);
-    sk = __reduce_add_sync(0xffffffffu, sk);
-    if ((threadIdx.x & 31) == 0) {
-        atomicAdd(&sh_stats[0], c);
-        atomicAdd(&sh_stats[1], sk);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        atomicAdd(p.stats + 0, (unsigned long long)sh_stats[0]);
-        atomicAdd(p.stats + 1, (unsigned long long)sh_stats[1]);
-    }
+    flush_stats(lg == 0 ? n_correct : 0u, lg == 0 ? n_skipped : 0u, p.stats);      // one count per group
 }
 
 // ---------------------------------------------------------------------------------------
-// Chunked variant (the default): the per-sample bookkeeping that every lane of a group used
-// to compute redundantly (Philox, range reduction, pair gather, key hash, bucket probe) is done
-// ONCE PER LANE FOR G DIFFERENT SAMPLES -- lane l of a group resolves sample (chunk*G + l) --
-// so a group has G independent metadata gathers in flight at once and pays 1/G of those
-// instructions per sample.  The G resolved triplets are then broadcast one by one with warp
-// shuffles and applied by the whole group (row gathers of sample t+1 are issued before the
-// arithmetic of sample t).
-template <int G, int NPL, bool VEC, bool ATOMIC, int MINB, int DEPTH>
+// Chunked kernel (the layouts with up to 8 floats of a row per lane, but for the one of the streamed kernel below): the
+// per-sample bookkeeping that every lane of a group would compute redundantly (Philox, range reduction, pair gather, key
+// hash, bucket probe) is done ONCE PER LANE FOR G DIFFERENT SAMPLES -- lane l of a group resolves sample (chunk*G + l) --
+// so a group has G independent metadata gathers in flight at once and pays 1/G of those instructions per sample.  The G
+// resolved triplets are then broadcast one by one with warp shuffles and applied by the whole group, DEPTH row-gathers
+// ahead of the arithmetic: groups of fewer than 32 lanes two gathers ahead at 3 resident blocks per SM, 32-lane groups one
+// ahead at 4.
+template <int G, int NPL, bool VEC, bool ATOMIC, int MINB = (G < 32 ? 3 : 4), int DEPTH = (G < 32 ? 2 : 1)>
 __global__ void __launch_bounds__(256, MINB) bpr_hogwild_chunk_kernel(const BprParams p)
 {
     using Frag = RowFrag<NPL, VEC>;
@@ -243,7 +274,6 @@ __global__ void __launch_bounds__(256, MINB) bpr_hogwild_chunk_kernel(const BprP
     const int64_t gid = (int64_t)blockIdx.x * groups_per_block + threadIdx.x / G;
     const int64_t n_chunks = (p.n_samples + G - 1) / G;
     const size_t k = (size_t)p.k;
-    const float lr = p.lr, reg = p.reg;
 
     unsigned int n_correct = 0, n_skipped = 0;
 
@@ -251,26 +281,14 @@ __global__ void __launch_bounds__(256, MINB) bpr_hogwild_chunk_kernel(const BprP
         // ---- phase 1: this lane's own sample
         const int64_t sl = c * G + lg;
         int mlive = sl < p.n_samples;
-        const uint64_t s = p.sample_base + (uint64_t)sl;
-        const Philox4 r = philox4x32_10((uint32_t)s, (uint32_t)(s >> 32), p.epoch_lo, p.epoch_hi, p.seed_lo, p.seed_hi);
-        int64_t i_lo, i_len, j_lo, j_len;
-        law_ranges(p.law, s, i_lo, i_len, j_lo, j_len);
-        const int64_t ii = i_lo + (int64_t)range64(r.x, r.y, (uint64_t)i_len);
-        const int32_t mj = p.neg_weighted ? __ldg(p.pairs + range64(r.z, r.w, (uint64_t)p.nnz)).y     // recom_wbpr.pyx:131
-                                          : (int32_t)(j_lo + (int64_t)range64(r.z, r.w, (uint64_t)j_len));
+        int64_t ii;
+        int32_t mj;
+        draw_sample(p, sl, ii, mj);
         const int2 pr = __ldg(p.pairs + ii);
         const int32_t mu = pr.x, mi = pr.y;
         {
-            const uint64_t key = ((uint64_t)(uint32_t)mu << 32) | (uint32_t)mj;
-            uint64_t bb = mix64(key) & p.bucket_mask;
-            bool found, full;
-            do {
-                const ulonglong2 b0 = __ldg(reinterpret_cast<const ulonglong2*>(p.table + 4 * bb));
-                const ulonglong2 b1 = __ldg(reinterpret_cast<const ulonglong2*>(p.table + 4 * bb) + 1);
-                found = (b0.x == key) | (b0.y == key) | (b1.x == key) | (b1.y == key);
-                full = (b1.y != TABLE_EMPTY);
-                bb = (bb + 1) & p.bucket_mask;
-            } while (!found && full);              // rare: the bucket overflowed into the next one
+            const uint64_t key = pair_key(mu, mj);
+            const bool found = bucket_has(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask);
             if (mlive && found) { mlive = 0; ++n_skipped; }          // recom_bpr.pyx:241-243
         }
         // ---- phase 2: apply the G samples one after the other, DEPTH row-gathers ahead
@@ -305,77 +323,22 @@ __global__ void __launch_bounds__(256, MINB) bpr_hogwild_chunk_kernel(const BprP
             for (int e = 0; e < E; ++e) part = fmaf(fu[cur].v[e], fi[cur].v[e] - fj[cur].v[e], part);
             const float score = (bi[cur] - bj[cur]) + group_sum<G>(part);      // recom_bpr.pyx:249-251
             float z;
-            if (p.hinge) {                              // recom_mmmf.pyx:137-139
-                if (score > 0.f) { ++n_correct; continue; }
-                z = 1.f;
-            } else {
-                z = bpr_z(score, p.exact_exp);
-                n_correct += (z < .5f);
-            }
-            float* pu = p.U + (size_t)cu[cur] * k;
-            float* pi = p.V + (size_t)ci[cur] * k;
-            float* pj = p.V + (size_t)cj[cur] * k;
-            if (ATOMIC) {
-                Frag du, di, dj;
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const float uf = fu[cur].v[e], vi = fi[cur].v[e], vj = fj[cur].v[e];
-                    du.v[e] = lr * (z * (vi - vj) - reg * uf);
-                    di.v[e] = lr * (z * uf - reg * vi);
-                    dj.v[e] = lr * (-z * uf - reg * vj);
-                }
-                if (!(p.debug_skip & 1)) row_red_add<G, NPL, VEC>(du, pu, lg, n_units);
-                if (!(p.debug_skip & 2)) row_red_add<G, NPL, VEC>(di, pi, lg, n_units);
-                if (!(p.debug_skip & 4)) row_red_add<G, NPL, VEC>(dj, pj, lg, n_units);
-                if (p.use_bias && lg == 0) {
-                    red_add_f32(p.B + ci[cur], lr * (z - reg * bi[cur]));
-                    red_add_f32(p.B + cj[cur], lr * (-z - reg * bj[cur]));
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const float uf = fu[cur].v[e], vi = fi[cur].v[e], vj = fj[cur].v[e];
-                    fu[cur].v[e] = uf + lr * (z * (vi - vj) - reg * uf);
-                    fi[cur].v[e] = vi + lr * (z * uf - reg * vi);
-                    fj[cur].v[e] = vj + lr * (-z * uf - reg * vj);
-                }
-                row_store<G, NPL, VEC>(fu[cur], pu, lg, n_units);
-                row_store<G, NPL, VEC>(fi[cur], pi, lg, n_units);
-                row_store<G, NPL, VEC>(fj[cur], pj, lg, n_units);
-                if (p.use_bias && lg == 0) {
-                    __stcg(p.B + ci[cur], bi[cur] + lr * (z - reg * bi[cur]));
-                    __stcg(p.B + cj[cur], bj[cur] + lr * (-z - reg * bj[cur]));
-                }
-            }
+            if (!sample_z(p.hinge, p.exact_exp, score, z, n_correct)) continue;
+            frag_update<G, NPL, VEC, ATOMIC>(p, fu[cur], fi[cur], fj[cur], bi[cur], bj[cur], cu[cur], ci[cur], cj[cur], z,
+                                             lg, n_units);
         }
     }
-
-    __shared__ unsigned int sh_stats[2];
-    if (threadIdx.x < 2) sh_stats[threadIdx.x] = 0;
-    __syncthreads();
-    unsigned int cc = (lg == 0) ? n_correct : 0u, sk = n_skipped;     // skips were counted per lane
-    cc = __reduce_add_sync(0xffffffffu, cc);
-    sk = __reduce_add_sync(0xffffffffu, sk);
-    if (lane == 0) {
-        atomicAdd(&sh_stats[0], cc);
-        atomicAdd(&sh_stats[1], sk);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        atomicAdd(p.stats + 0, (unsigned long long)sh_stats[0]);
-        atomicAdd(p.stats + 1, (unsigned long long)sh_stats[1]);
-    }
+    flush_stats(lg == 0 ? n_correct : 0u, n_skipped, p.stats);      // skips were counted per lane
 }
 
 // ---------------------------------------------------------------------------------------
-// Streamed variant (the default for k % 4 == 0, k <= 128): the chunked kernel above keeps the rows of the samples in
-// flight in REGISTERS (one sample ahead: 24 registers), is fully unrolled over the G samples of a chunk (190 KB of code:
-// 17 % of its stall samples were instruction-cache misses, ncu r02) and exposes the two dependent DRAM gathers of the
-// sampling (pair -> bucket) once per chunk.  Here
+// Streamed kernel (k % 4 == 0, 64 < k <= 128: 32-lane groups, one float4 of a row per lane): the chunked kernel above keeps
+// the rows of the samples in flight in REGISTERS, is fully unrolled over the G samples of a chunk (190 KB of code: 17 % of
+// its stall samples were instruction-cache misses, ncu r02) and exposes the two dependent DRAM gathers of the sampling
+// (pair -> bucket) once per chunk.  Here
 //   * the factor rows of the next D samples are staged in SHARED MEMORY with cp.async (LDGSTS.BYPASS, L2-coherent like
 //     the ld.global.cg they replace): every lane copies and later reads back only its own 16-byte column, so no barrier
-//     is needed, no register is held by a row in flight, and D = 4 samples (6 KB per warp at k = 128) are in flight
-//     per group instead of 2;
+//     is needed and no register is held by a row in flight;
 //   * the sampling of the NEXT chunk (Philox, pair gather, membership bucket) is issued while the current chunk's
 //     samples are applied, one step per quarter of the chunk, so its latency is off the critical path;
 //   * the loop over the chunk is a real loop (unrolled by 2), the per-sample integer work is cut down (triplet packed
@@ -408,19 +371,14 @@ __device__ __forceinline__ void meta_step_a(const BprParams& p, ChunkMeta& m, in
 {
     const int64_t sl = chunk * G + lg;
     m.in_range = sl < p.n_samples;
-    const uint64_t s = p.sample_base + (uint64_t)sl;
-    const Philox4 r = philox4x32_10((uint32_t)s, (uint32_t)(s >> 32), p.epoch_lo, p.epoch_hi, p.seed_lo, p.seed_hi);
-    int64_t i_lo, i_len, j_lo, j_len;
-    law_ranges(p.law, s, i_lo, i_len, j_lo, j_len);
-    const int64_t ii = i_lo + (int64_t)range64(r.x, r.y, (uint64_t)i_len);
-    m.j = p.neg_weighted ? __ldg(p.pairs + range64(r.z, r.w, (uint64_t)p.nnz)).y     // recom_wbpr.pyx:131
-                         : (int32_t)(j_lo + (int64_t)range64(r.z, r.w, (uint64_t)j_len));
+    int64_t ii;
+    draw_sample(p, sl, ii, m.j);
     m.pr = __ldg(p.pairs + ii);
 }
 __device__ __forceinline__ void meta_step_b(const BprParams& p, ChunkMeta& m)
 {
     m.u = m.pr.x; m.i = m.pr.y;
-    m.key = ((uint64_t)(uint32_t)m.u << 32) | (uint32_t)m.j;
+    m.key = pair_key(m.u, m.j);
     m.bucket = mix64(m.key) & p.bucket_mask;
     m.b0 = __ldg(reinterpret_cast<const ulonglong2*>(p.table + 4 * m.bucket));
     m.b1 = __ldg(reinterpret_cast<const ulonglong2*>(p.table + 4 * m.bucket) + 1);
@@ -429,15 +387,8 @@ __device__ __forceinline__ void meta_step_b(const BprParams& p, ChunkMeta& m)
 __device__ __forceinline__ int meta_step_c(const BprParams& p, ChunkMeta& m)
 {
     bool found = (m.b0.x == m.key) | (m.b0.y == m.key) | (m.b1.x == m.key) | (m.b1.y == m.key);
-    bool full = (m.b1.y != TABLE_EMPTY);
-    uint64_t bb = m.bucket;
-    while (!found && full) {                    // rare: the bucket overflowed into the next one
-        bb = (bb + 1) & p.bucket_mask;
-        const ulonglong2 c0 = __ldg(reinterpret_cast<const ulonglong2*>(p.table + 4 * bb));
-        const ulonglong2 c1 = __ldg(reinterpret_cast<const ulonglong2*>(p.table + 4 * bb) + 1);
-        found = (c0.x == m.key) | (c0.y == m.key) | (c1.x == m.key) | (c1.y == m.key);
-        full = (c1.y != TABLE_EMPTY);
-    }
+    if (!found && m.b1.y != TABLE_EMPTY)        // rare: the bucket overflowed into the next one
+        found = bucket_has(p.table, p.bucket_mask, m.key, (m.bucket + 1) & p.bucket_mask);
     const int skipped = m.in_range && found;
     if (!m.in_range || found) m.u = ~m.u;      // u >= 0 always: the complement is negative = "not live"
     return skipped;
@@ -525,25 +476,16 @@ __global__ void __launch_bounds__(256, MINB) bpr_hogwild_stream_kernel(const Bpr
             part = fmaf(u4.y, dy, part); part = fmaf(u4.z, dz, part); part = fmaf(u4.w, dw, part);
             const float score = (bi - bj) + group_sum<G>(part);       // recom_bpr.pyx:249-251
             float z;
-            if (p.hinge) {                              // recom_mmmf.pyx:137-139
-                if (score > 0.f) { ++n_correct; continue; }
-                z = 1.f;
-            } else {
-                z = bpr_z(score, p.exact_exp);
-                n_correct += (z < .5f);
-            }
+            if (!sample_z(p.hinge, p.exact_exp, score, z, n_correct)) continue;
             const float a = lr * z;                     // delta = lr (z x - reg y) = a x - lrreg y
             float* pu = p.U + (size_t)su * k + lg * 4;
             float* pi = p.V + (size_t)si * k + lg * 4;
             float* pj = p.V + (size_t)sj * k + lg * 4;
             if (col) {
                 if (ATOMIC) {
-                    if (!(p.debug_skip & 1))
-                        red_add_v4(pu, fmaf(a, dx, -lrreg * u4.x), fmaf(a, dy, -lrreg * u4.y), fmaf(a, dz, -lrreg * u4.z), fmaf(a, dw, -lrreg * u4.w));
-                    if (!(p.debug_skip & 2))
-                        red_add_v4(pi, fmaf(a, u4.x, -lrreg * vi4.x), fmaf(a, u4.y, -lrreg * vi4.y), fmaf(a, u4.z, -lrreg * vi4.z), fmaf(a, u4.w, -lrreg * vi4.w));
-                    if (!(p.debug_skip & 4))
-                        red_add_v4(pj, fmaf(-a, u4.x, -lrreg * vj4.x), fmaf(-a, u4.y, -lrreg * vj4.y), fmaf(-a, u4.z, -lrreg * vj4.z), fmaf(-a, u4.w, -lrreg * vj4.w));
+                    red_add_v4(pu, fmaf(a, dx, -lrreg * u4.x), fmaf(a, dy, -lrreg * u4.y), fmaf(a, dz, -lrreg * u4.z), fmaf(a, dw, -lrreg * u4.w));
+                    red_add_v4(pi, fmaf(a, u4.x, -lrreg * vi4.x), fmaf(a, u4.y, -lrreg * vi4.y), fmaf(a, u4.z, -lrreg * vi4.z), fmaf(a, u4.w, -lrreg * vi4.w));
+                    red_add_v4(pj, fmaf(-a, u4.x, -lrreg * vj4.x), fmaf(-a, u4.y, -lrreg * vj4.y), fmaf(-a, u4.z, -lrreg * vj4.z), fmaf(-a, u4.w, -lrreg * vj4.w));
                 } else {
                     __stcg(reinterpret_cast<float4*>(pu), make_float4(u4.x + fmaf(a, dx, -lrreg * u4.x), u4.y + fmaf(a, dy, -lrreg * u4.y),
                                                                       u4.z + fmaf(a, dz, -lrreg * u4.z), u4.w + fmaf(a, dw, -lrreg * u4.w)));
@@ -566,27 +508,11 @@ __global__ void __launch_bounds__(256, MINB) bpr_hogwild_stream_kernel(const Bpr
         cur = nxt;
     }
     cp_async_wait<0>();
-
-    __shared__ unsigned int sh_stats[2];
-    if (threadIdx.x < 2) sh_stats[threadIdx.x] = 0;
-    __syncthreads();
-    unsigned int cc = (lg == 0) ? n_correct : 0u, sk = n_skipped;     // skips were counted per lane
-    cc = __reduce_add_sync(0xffffffffu, cc);
-    sk = __reduce_add_sync(0xffffffffu, sk);
-    if (lane == 0) {
-        atomicAdd(&sh_stats[0], cc);
-        atomicAdd(&sh_stats[1], sk);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        atomicAdd(p.stats + 0, (unsigned long long)sh_stats[0]);
-        atomicAdd(p.stats + 1, (unsigned long long)sh_stats[1]);
-    }
+    flush_stats(lg == 0 ? n_correct : 0u, n_skipped, p.stats);      // skips were counted per lane
 }
 
 // ---------------------------------------------------------------------------------------
-// Parity mode: one warp, serial-equivalent.  Unfused f32 arithmetic in the operation order
-// of recom_bpr.pyx:249-267 (the dot is a lane-strided partial sum + shuffle tree).
+// Parity mode: the sample stream is applied with the result of the strictly serial loop, bit for bit.
 struct ReplayParams {
     const int64_t* __restrict__ i_index;
     const int32_t* __restrict__ j_id;
@@ -604,10 +530,65 @@ struct ReplayParams {
     unsigned long long* stats;
 };
 
+// One sample (u, i, j) on one warp: unfused f32 arithmetic in the operation order of recom_bpr.pyx:249-267 (the dot is a
+// lane-strided partial sum over f = lane, lane + 32, ... + shuffle tree).  The first RC elements per lane stay in
+// registers between the dot and the update (k <= 128: the rows are read once per sample instead of twice).  ld / st
+// read and write the factors U, V, B: in global memory or an on-chip copy.  Returns 1 when the sample counts as
+// correctly ranked (every lane returns the same).
+template <class Ld, class St>
+__device__ __forceinline__ int replay_sample(const ReplayParams& p, float* U, float* V, float* B, int32_t u, int32_t i,
+                                             int32_t j, int lane, Ld ld, St st)
+{
+    const size_t k = (size_t)p.k;
+    float* pu = U + (size_t)u * k;
+    float* pi = V + (size_t)i * k;
+    float* pj = V + (size_t)j * k;
+    const float bi = ld(B + i), bj = ld(B + j);
+    constexpr int RC = 4;
+    float ru[RC], ri[RC], rj[RC];
+    float part = 0.f;
+#pragma unroll
+    for (int x = 0; x < RC; ++x) {
+        const int f = lane + 32 * x;
+        ru[x] = ri[x] = rj[x] = 0.f;
+        if (f < p.k) { ru[x] = ld(pu + f); ri[x] = ld(pi + f); rj[x] = ld(pj + f); }
+    }
+#pragma unroll
+    for (int x = 0; x < RC; ++x)
+        if (lane + 32 * x < p.k) part = __fadd_rn(part, __fmul_rn(ru[x], __fsub_rn(ri[x], rj[x])));
+    for (int f = lane + 32 * RC; f < p.k; f += 32)
+        part = __fadd_rn(part, __fmul_rn(ld(pu + f), __fsub_rn(ld(pi + f), ld(pj + f))));
+    const float score = __fadd_rn(__fsub_rn(bi, bj), group_sum<32>(part));
+    float z;
+    int correct = 0;
+    if (sample_z(p.hinge, 1, score, z, correct)) {
+        const float lr = p.lr, reg = p.reg;
+        auto step = [&](int f, float uf, float vi, float vj) {
+            st(pu + f, __fadd_rn(uf, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, __fsub_rn(vi, vj)), __fmul_rn(reg, uf)))));
+            st(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, uf), __fmul_rn(reg, vi)))));
+            st(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-z, uf), __fmul_rn(reg, vj)))));
+        };
+#pragma unroll
+        for (int x = 0; x < RC; ++x)
+            if (lane + 32 * x < p.k) step(lane + 32 * x, ru[x], ri[x], rj[x]);
+        for (int f = lane + 32 * RC; f < p.k; f += 32) {
+            const float uf = ld(pu + f), vi = ld(pi + f), vj = ld(pj + f);
+            step(f, uf, vi, vj);
+        }
+        if (p.use_bias && lane == 0) {
+            st(B + i, __fadd_rn(bi, __fmul_rn(lr, __fsub_rn(z, __fmul_rn(reg, bi)))));
+            st(B + j, __fadd_rn(bj, __fmul_rn(lr, __fsub_rn(-z, __fmul_rn(reg, bj)))));
+        }
+    }
+    return correct;
+}
+
+// The strictly serial reference: one warp, the samples one after the other
 __global__ void __launch_bounds__(32) bpr_replay_kernel(const ReplayParams p)
 {
     const int lane = threadIdx.x;
-    const size_t k = (size_t)p.k;
+    auto ld = [](const float* a) { return __ldcg(a); };
+    auto st = [](float* a, float v) { __stcg(a, v); };
     unsigned long long n_correct = 0, n_skipped = 0;
     for (int64_t base = 0; base < p.n_samples; base += 32) {
         // metadata of 32 consecutive samples, one per lane (read-only inputs => order-free)
@@ -628,33 +609,7 @@ __global__ void __launch_bounds__(32) bpr_replay_kernel(const ReplayParams p)
             const int32_t u = __shfl_sync(0xffffffffu, mu, t);
             const int32_t i = __shfl_sync(0xffffffffu, mi, t);
             const int32_t j = __shfl_sync(0xffffffffu, mj, t);
-            float* pu = p.U + (size_t)u * k;
-            float* pi = p.V + (size_t)i * k;
-            float* pj = p.V + (size_t)j * k;
-            const float bi = __ldcg(p.B + i), bj = __ldcg(p.B + j);
-            float part = 0.f;
-            for (int f = lane; f < p.k; f += 32)
-                part = __fadd_rn(part, __fmul_rn(__ldcg(pu + f), __fsub_rn(__ldcg(pi + f), __ldcg(pj + f))));
-            const float score = __fadd_rn(__fsub_rn(bi, bj), group_sum<32>(part));
-            float z;
-            if (p.hinge) {                              // recom_mmmf.pyx:137-139 (warp-uniform)
-                if (score > 0.f) { ++n_correct; continue; }
-                z = 1.f;
-            } else {
-                z = (float)(1.0 / (1.0 + exp((double)score)));
-                n_correct += (z < .5f);
-            }
-            const float lr = p.lr, reg = p.reg;
-            for (int f = lane; f < p.k; f += 32) {
-                const float uf = __ldcg(pu + f), vi = __ldcg(pi + f), vj = __ldcg(pj + f);
-                __stcg(pu + f, __fadd_rn(uf, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, __fsub_rn(vi, vj)), __fmul_rn(reg, uf)))));
-                __stcg(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, uf), __fmul_rn(reg, vi)))));
-                __stcg(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-z, uf), __fmul_rn(reg, vj)))));
-            }
-            if (p.use_bias && lane == 0) {
-                __stcg(p.B + i, __fadd_rn(bi, __fmul_rn(lr, __fsub_rn(z, __fmul_rn(reg, bi)))));
-                __stcg(p.B + j, __fadd_rn(bj, __fmul_rn(lr, __fsub_rn(-z, __fmul_rn(reg, bj)))));
-            }
+            n_correct += replay_sample(p, p.U, p.V, p.B, u, i, j, lane, ld, st);
             __syncwarp();   // order lane 0's bias stores before the next sample's reads
         }
     }
@@ -678,7 +633,7 @@ __global__ void bpr_prepare_kernel(const int32_t* __restrict__ indptr, const int
         for (int64_t e = lo + lane; e < hi; e += 32) {
             const int32_t i = __ldg(indices + e);
             pairs[e] = make_int2((int32_t)u, i);                    // COO row = user_ids of recom_bpr.pyx:154-161
-            const unsigned long long key = ((unsigned long long)(uint32_t)u << 32) | (uint32_t)i;
+            const unsigned long long key = pair_key((int32_t)u, i);
             uint64_t b = mix64(key) & bucket_mask;
             for (;;) {
                 bool done = false;
@@ -701,141 +656,10 @@ static int64_t table_buckets_for(int64_t nnz)
     return b;
 }
 
-struct HogwildTune {
-    int S, threads, blocks_per_sm;
-};
-static HogwildTune read_tune()
-{
-    HogwildTune t{0, 256, 0};
-    if (const char* e = getenv("B200_BPR_TUNE")) sscanf(e, "%d,%d,%d", &t.S, &t.threads, &t.blocks_per_sm);
-    if (t.threads != 64 && t.threads != 128 && t.threads != 256) t.threads = 256;
-    return t;
-}
-
-// ---------------------------------------------------------------------------------------
-// Parity mode, windowed: one CTA of 32 warps.  32 consecutive samples are resolved at a time (one per
-// warp) and executed in dependency order: a sample may run as soon as no EARLIER still-pending sample
-// of the window touches one of its rows (its user row, or either of its two item rows).  Samples that
-// share no row commute exactly, so the result is bit-identical to bpr_replay_kernel (strictly serial)
-// while independent samples run in parallel -- on a matrix with thousands of rows a window needs 1-3
-// rounds instead of 32 serial updates.
-__global__ void __launch_bounds__(1024) bpr_replay_window_kernel(const ReplayParams p)
-{
-    __shared__ int m_u[1024], m_i[1024], m_j[1024];
-    __shared__ unsigned char m_todo[1024];
-    __shared__ int s_u[32], s_i[32], s_j[32], s_pending[32];
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const size_t k = (size_t)p.k;
-    unsigned long long n_correct = 0, n_skipped = 0;
-    for (int64_t base0 = 0; base0 < p.n_samples; base0 += 1024) {
-        // ---- resolve 1024 samples at once, one per THREAD (read-only inputs => order-free): the ~10
-        //      dependent gathers of (u, i, skip test) are paid once per 32 windows
-        __syncthreads();
-        {
-            const int64_t s = base0 + threadIdx.x;
-            int32_t mu = 0, mi = 0, mj = 0;
-            bool todo = false;
-            if (s < p.n_samples) {
-                const int64_t ii = p.i_index[s];
-                mj = p.j_id[s];
-                mu = __ldg(p.coo_row + ii);
-                mi = __ldg(p.indices + ii);
-                todo = !row_contains(p.indices, __ldg(p.indptr + mu), __ldg(p.indptr + mu + 1), mj);
-                if (!todo) ++n_skipped;             // counted per thread, summed at the end
-            }
-            m_u[threadIdx.x] = mu; m_i[threadIdx.x] = mi; m_j[threadIdx.x] = mj; m_todo[threadIdx.x] = todo ? 1 : 0;
-        }
-        __syncthreads();
-        const int n_win = (int)min((int64_t)32, (p.n_samples - base0 + 31) / 32);
-      for (int win = 0; win < n_win; ++win) {
-        const int slot = win * 32 + w;              // this warp's sample of the window
-        const int32_t mu = m_u[slot], mi = m_i[slot], mj = m_j[slot];
-        bool todo = m_todo[slot] != 0;
-        __syncthreads();                            // previous window fully retired
-        if (lane == 0) { s_u[w] = mu; s_i[w] = mi; s_j[w] = mj; s_pending[w] = todo ? 1 : 0; }
-        for (;;) {
-            if (!__syncthreads_or(todo)) break;     // also publishes the state written in the last round
-            bool run = false;
-            if (todo) {
-                bool conflict = false;
-                if (lane < w && s_pending[lane]) {
-                    const int ou = s_u[lane], oi = s_i[lane], oj = s_j[lane];
-                    conflict = (ou == mu) | (oi == mi) | (oi == mj) | (oj == mi) | (oj == mj);
-                }
-                run = !__any_sync(0xffffffffu, conflict);
-            }
-            __syncthreads();                        // everybody has read the snapshot of s_pending
-            if (run) {
-                float* pu = p.U + (size_t)mu * k;
-                float* pi = p.V + (size_t)mi * k;
-                float* pj = p.V + (size_t)mj * k;
-                const float bi = __ldcg(p.B + mi), bj = __ldcg(p.B + mj);
-                // the first RC elements per lane stay in registers between the dot and the update (k <= 128:
-                // the rows are read from L2 once per sample instead of twice)
-                constexpr int RC = 4;
-                float ru[RC], ri[RC], rj[RC];
-                float part = 0.f;
-#pragma unroll
-                for (int t = 0; t < RC; ++t) {
-                    const int f = lane + 32 * t;
-                    ru[t] = ri[t] = rj[t] = 0.f;
-                    if (f < p.k) { ru[t] = __ldcg(pu + f); ri[t] = __ldcg(pi + f); rj[t] = __ldcg(pj + f); }
-                }
-#pragma unroll
-                for (int t = 0; t < RC; ++t)
-                    if (lane + 32 * t < p.k) part = __fadd_rn(part, __fmul_rn(ru[t], __fsub_rn(ri[t], rj[t])));
-                for (int f = lane + 32 * RC; f < p.k; f += 32)
-                    part = __fadd_rn(part, __fmul_rn(__ldcg(pu + f), __fsub_rn(__ldcg(pi + f), __ldcg(pj + f))));
-                const float score = __fadd_rn(__fsub_rn(bi, bj), group_sum<32>(part));
-                float z = 1.f;
-                bool update = true;
-                if (p.hinge) {                      // recom_mmmf.pyx:137-139
-                    if (score > 0.f) { ++n_correct; update = false; }
-                } else {
-                    z = (float)(1.0 / (1.0 + exp((double)score)));
-                    n_correct += (z < .5f);
-                }
-                if (update) {
-                    const float lr = p.lr, reg = p.reg;
-#pragma unroll
-                    for (int t = 0; t < RC; ++t) {
-                        const int f = lane + 32 * t;
-                        if (f < p.k) {
-                            const float uf = ru[t], vi = ri[t], vj = rj[t];
-                            __stcg(pu + f, __fadd_rn(uf, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, __fsub_rn(vi, vj)), __fmul_rn(reg, uf)))));
-                            __stcg(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, uf), __fmul_rn(reg, vi)))));
-                            __stcg(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-z, uf), __fmul_rn(reg, vj)))));
-                        }
-                    }
-                    for (int f = lane + 32 * RC; f < p.k; f += 32) {
-                        const float uf = __ldcg(pu + f), vi = __ldcg(pi + f), vj = __ldcg(pj + f);
-                        __stcg(pu + f, __fadd_rn(uf, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, __fsub_rn(vi, vj)), __fmul_rn(reg, uf)))));
-                        __stcg(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, uf), __fmul_rn(reg, vi)))));
-                        __stcg(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-z, uf), __fmul_rn(reg, vj)))));
-                    }
-                    if (p.use_bias && lane == 0) {
-                        __stcg(p.B + mi, __fadd_rn(bi, __fmul_rn(lr, __fsub_rn(z, __fmul_rn(reg, bi)))));
-                        __stcg(p.B + mj, __fadd_rn(bj, __fmul_rn(lr, __fsub_rn(-z, __fmul_rn(reg, bj)))));
-                    }
-                }
-                todo = false;
-                if (lane == 0) s_pending[w] = 0;
-            }
-        }
-      }
-    }
-    // correct: one count per warp (lane 0); skipped: one count per resolving thread
-    const unsigned long long sk = __reduce_add_sync(0xffffffffu, (unsigned)n_skipped);
-    if (lane == 0) {
-        atomicAdd(p.stats + 0, n_correct);
-        atomicAdd(p.stats + 1, sk);
-    }
-}
-
 // ---------------------------------------------------------------------------------------
 // Parity mode, scheduled: one CTA of 32 warps, dependencies resolved over whole PHASES of 1024 samples.
-// The windowed kernel above only looks 32 samples ahead; the stream's own critical path is 3-4x shorter than what
-// 32-sample windows allow (tools/replay_levels.py).  Here every thread owns one sample of the phase and, round by round,
+// The stream's critical path is far shorter than its length (tools/replay_levels.py).  Every thread owns one sample of
+// the phase and, round by round,
 //   (A) every pending sample puts its index into the slots of its three rows in two direct-mapped "earliest pending
 //       toucher" tables (atomicMin; user rows and item rows apart);
 //   (B) a sample that holds all three of its slots has no earlier pending sample on any of its rows: it is READY.  Hash
@@ -864,7 +688,6 @@ __global__ void __launch_bounds__(1024) bpr_replay_sched_kernel(const ReplayPara
     float* sV = sU + (SMEM_MODEL ? n_users * p.k : 0);
     float* sB = sV + (SMEM_MODEL ? n_items * p.k : 0);
     const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
-    const size_t k = (size_t)p.k;
     if (SMEM_MODEL) {
         for (int64_t x = tid; x < n_users * p.k; x += 1024) sU[x] = __ldcg(p.U + x);
         for (int64_t x = tid; x < n_items * p.k; x += 1024) sV[x] = __ldcg(p.V + x);
@@ -921,57 +744,7 @@ __global__ void __launch_bounds__(1024) bpr_replay_sched_kernel(const ReplayPara
             const int n_ready = sh.q_n;
             for (int q = w; q < n_ready; q += 32) {
                 const int t = sh.queue[q];
-                const int32_t u = sh.m_u[t], i = sh.m_i[t], j = sh.m_j[t];
-                float* pu = Ub + (size_t)u * k;
-                float* pi = Vb + (size_t)i * k;
-                float* pj = Vb + (size_t)j * k;
-                const float bi = ld(Bb + i), bj = ld(Bb + j);
-                constexpr int RC = 4;                              // k <= 128: rows stay in registers between dot and update
-                float ru[RC], ri[RC], rj[RC];
-                float part = 0.f;
-#pragma unroll
-                for (int x = 0; x < RC; ++x) {
-                    const int f = lane + 32 * x;
-                    ru[x] = ri[x] = rj[x] = 0.f;
-                    if (f < p.k) { ru[x] = ld(pu + f); ri[x] = ld(pi + f); rj[x] = ld(pj + f); }
-                }
-#pragma unroll
-                for (int x = 0; x < RC; ++x)
-                    if (lane + 32 * x < p.k) part = __fadd_rn(part, __fmul_rn(ru[x], __fsub_rn(ri[x], rj[x])));
-                for (int f = lane + 32 * RC; f < p.k; f += 32)
-                    part = __fadd_rn(part, __fmul_rn(ld(pu + f), __fsub_rn(ld(pi + f), ld(pj + f))));
-                const float score = __fadd_rn(__fsub_rn(bi, bj), group_sum<32>(part));
-                float z = 1.f;
-                bool update = true;
-                if (p.hinge) {                                     // recom_mmmf.pyx:137-139
-                    if (score > 0.f) { ++n_correct; update = false; }
-                } else {
-                    z = (float)(1.0 / (1.0 + exp((double)score)));
-                    n_correct += (z < .5f);
-                }
-                if (update) {
-                    const float lr = p.lr, reg = p.reg;
-#pragma unroll
-                    for (int x = 0; x < RC; ++x) {
-                        const int f = lane + 32 * x;
-                        if (f < p.k) {
-                            const float uf = ru[x], vi = ri[x], vj = rj[x];
-                            st(pu + f, __fadd_rn(uf, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, __fsub_rn(vi, vj)), __fmul_rn(reg, uf)))));
-                            st(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, uf), __fmul_rn(reg, vi)))));
-                            st(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-z, uf), __fmul_rn(reg, vj)))));
-                        }
-                    }
-                    for (int f = lane + 32 * RC; f < p.k; f += 32) {
-                        const float uf = ld(pu + f), vi = ld(pi + f), vj = ld(pj + f);
-                        st(pu + f, __fadd_rn(uf, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, __fsub_rn(vi, vj)), __fmul_rn(reg, uf)))));
-                        st(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(z, uf), __fmul_rn(reg, vi)))));
-                        st(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-z, uf), __fmul_rn(reg, vj)))));
-                    }
-                    if (p.use_bias && lane == 0) {
-                        st(Bb + i, __fadd_rn(bi, __fmul_rn(lr, __fsub_rn(z, __fmul_rn(reg, bi)))));
-                        st(Bb + j, __fadd_rn(bj, __fmul_rn(lr, __fsub_rn(-z, __fmul_rn(reg, bj)))));
-                    }
-                }
+                n_correct += replay_sample(p, Ub, Vb, Bb, sh.m_u[t], sh.m_i[t], sh.m_j[t], lane, ld, st);
             }
             __syncthreads();                                       // queue consumed
             if (tid == 0) sh.q_n = 0;
@@ -991,70 +764,24 @@ __global__ void __launch_bounds__(1024) bpr_replay_sched_kernel(const ReplayPara
     }
 }
 
-template <int G, int NPL, bool VEC, bool ATOMIC, int S, int MINB>
-static int launch_hogwild_s(const BprParams& p, cudaStream_t st, const HogwildTune& tune)
+// Persistent grid of 256-thread blocks of G-lane groups: as many blocks as are resident on the device at once, but no
+// more than `units` units of work (one per group and grid-stride step) need, and no more groups than `max_groups`.  That
+// is the Hogwild staleness bound: never run more samples concurrently than a quarter of the rows of the smaller factor
+// matrix (with fewer rows than in-flight samples every update would be computed from a stale row and the epoch
+// degenerates into one huge-batch step).
+template <class Kern>
+static int launch_persistent(Kern kern, const BprParams& p, int G, int64_t units, int64_t max_groups, size_t smem,
+                             cudaStream_t st)
 {
-    auto kern = bpr_hogwild_kernel<G, NPL, VEC, ATOMIC, S, MINB>;
-    const int threads = tune.threads;
-    int occ = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0));
-    if (occ < 1) occ = 1;
-    if (tune.blocks_per_sm > 0 && tune.blocks_per_sm < occ) occ = tune.blocks_per_sm;
-    const int64_t groups_per_block = threads / G;
-    int64_t want = (p.n_samples + groups_per_block * S - 1) / (groups_per_block * S);
-    int64_t grid = (int64_t)sm_count() * occ;
-    if (want < grid) grid = want;
-    // Hogwild staleness bound: never run more samples concurrently than a quarter of the rows
-    // of the smaller factor matrix (with fewer rows than in-flight samples every update would
-    // be computed from a stale row and the epoch degenerates into one huge-batch step)
-    const int64_t cap = (p.max_groups + groups_per_block * S - 1) / (groups_per_block * S);
-    if (cap < grid) grid = cap;
-    if (grid < 1) grid = 1;
-    kern<<<(unsigned)grid, threads, 0, st>>>(p); ::b200::count_launch();
-    B200_CUDA(cudaGetLastError());
-    return B200_OK;
-}
-
-template <int G, int NPL, bool VEC, bool ATOMIC, int MINB, int DEPTH>
-static int launch_hogwild_chunk(const BprParams& p, cudaStream_t st, const HogwildTune& tune)
-{
-    auto kern = bpr_hogwild_chunk_kernel<G, NPL, VEC, ATOMIC, MINB, DEPTH>;
-    const int threads = tune.threads;
-    int occ = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0));
-    if (occ < 1) occ = 1;
-    if (tune.blocks_per_sm > 0 && tune.blocks_per_sm < occ) occ = tune.blocks_per_sm;
-    const int64_t groups_per_block = threads / G;
-    const int64_t n_chunks = (p.n_samples + G - 1) / G;
-    int64_t want = (n_chunks + groups_per_block - 1) / groups_per_block;
-    int64_t grid = (int64_t)sm_count() * occ;
-    if (want < grid) grid = want;
-    const int64_t cap = (p.max_groups + groups_per_block - 1) / groups_per_block;     // staleness bound
-    if (cap < grid) grid = cap;
-    if (grid < 1) grid = 1;
-    kern<<<(unsigned)grid, threads, 0, st>>>(p); ::b200::count_launch();
-    B200_CUDA(cudaGetLastError());
-    return B200_OK;
-}
-
-template <int G, bool ATOMIC, int D, int MINB>
-static int launch_hogwild_stream(const BprParams& p, cudaStream_t st, const HogwildTune& tune)
-{
-    auto kern = bpr_hogwild_stream_kernel<G, ATOMIC, D, MINB>;
-    const int threads = 256;
-    const size_t smem = (size_t)(threads / G) * D * (3 * G * 16);
-    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    constexpr int threads = 256;
     int occ = 0;
     B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
     if (occ < 1) occ = 1;
-    if (tune.blocks_per_sm > 0 && tune.blocks_per_sm < occ) occ = tune.blocks_per_sm;
     const int64_t groups_per_block = threads / G;
-    const int64_t n_chunks = (p.n_samples + G - 1) / G;
-    int64_t want = (n_chunks + groups_per_block - 1) / groups_per_block;
+    const int64_t want = (units + groups_per_block - 1) / groups_per_block;
+    const int64_t cap = (max_groups + groups_per_block - 1) / groups_per_block;
     int64_t grid = (int64_t)sm_count() * occ;
     if (want < grid) grid = want;
-    // staleness bound (see launch_hogwild_s): a group has D samples in flight
-    const int64_t cap = (p.max_groups / D + groups_per_block - 1) / groups_per_block;
     if (cap < grid) grid = cap;
     if (grid < 1) grid = 1;
     kern<<<(unsigned)grid, threads, smem, st>>>(p); ::b200::count_launch();
@@ -1062,35 +789,27 @@ static int launch_hogwild_stream(const BprParams& p, cudaStream_t st, const Hogw
     return B200_OK;
 }
 
+// One kernel per row layout (pick_layout), E floats of a row per lane.  The launch shapes were chosen on B200 and have
+// not been re-tuned on the H100.
 template <int G, int NPL, bool VEC, bool ATOMIC>
 static int launch_hogwild(const BprParams& p, cudaStream_t st)
 {
-    // samples in flight per group: bounded by the register footprint of the 3*S row fragments
     constexpr int E = NPL * (VEC ? 4 : 1);
-    const HogwildTune tune = read_tune();
-    if constexpr (VEC && NPL == 1 && G >= 16) {
-        // one float4 per lane (k % 4 == 0, 52 <= k <= 128): rows staged in shared memory, 2 samples in flight per group.
-        // 16-lane groups (k <= 64, V L2-resident at configs[1]) stay on the register-staged chunk kernel.
-        if (tune.S == 0 && G >= 32) return launch_hogwild_stream<G, ATOMIC, 2, 4>(p, st, tune);
-        if (tune.S == 2) return launch_hogwild_stream<G, ATOMIC, 2, 4>(p, st, tune);          // A/B: force the streamed kernels
-        if (tune.S == 4) return launch_hogwild_stream<G, ATOMIC, 4, 4>(p, st, tune);
-    }
-    if constexpr (E <= 8) {
-        // 16-lane groups run two row-gathers ahead at 3 blocks/SM; 32-lane groups (k = 128: 512-byte rows, V beyond the
-        // L2 at 1 M items) one gather ahead at 4 resident blocks (60 registers).  B200_BPR_TUNE selects the others.
-        if (tune.S == 0 || tune.S == 64) {       // (64 = the register-staged chunk kernel where the streamed one is the default)
-            if (G >= 32) return launch_hogwild_chunk<G, NPL, VEC, ATOMIC, 4, 1>(p, st, tune);
-            return launch_hogwild_chunk<G, NPL, VEC, ATOMIC, 3, 2>(p, st, tune);
-        }
-        if (tune.S == 32) {              // the other combinations, for A/B runs
-            if (G >= 32) return launch_hogwild_chunk<G, NPL, VEC, ATOMIC, 3, 1>(p, st, tune);
-            return launch_hogwild_chunk<G, NPL, VEC, ATOMIC, 4, 1>(p, st, tune);
-        }
-    }
-    if constexpr (E <= 4) {
-        return launch_hogwild_s<G, NPL, VEC, ATOMIC, 1, 5>(p, st, tune);      // register-only variant (B200_BPR_TUNE=1,...)
+    const int64_t n_chunks = (p.n_samples + G - 1) / G;
+    if constexpr (VEC && NPL == 1 && G == 32) {
+        // one float4 per lane (k % 4 == 0, 64 < k <= 128): rows staged in shared memory, D samples in flight per group
+        constexpr int D = 2;
+        auto kern = bpr_hogwild_stream_kernel<G, ATOMIC, D, 4>;
+        const size_t smem = (size_t)(256 / G) * D * (3 * G * 16);
+        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        return launch_persistent(kern, p, G, n_chunks, p.max_groups / D, smem, st);
+    } else if constexpr (E <= 8) {
+        return launch_persistent(bpr_hogwild_chunk_kernel<G, NPL, VEC, ATOMIC>, p, G, n_chunks, p.max_groups, 0, st);
     } else {
-        return launch_hogwild_s<G, NPL, VEC, ATOMIC, 1, hogwild_min_blocks<NPL, VEC, 1>()>(p, st, tune);
+        // 16 or 32 floats per lane: the resident blocks per SM the register allocator is asked to make room for (the
+        // kernel is latency-bound on dependent gathers, so samples in flight per SM is the lever)
+        return launch_persistent(bpr_hogwild_kernel<G, NPL, VEC, ATOMIC, (E <= 16 ? 2 : 1)>, p, G, p.n_samples,
+                                 p.max_groups, 0, st);
     }
 }
 
@@ -1131,13 +850,8 @@ __device__ __forceinline__ void det_apply(unsigned long long* a, float* x)
 // (u, i) and j of epoch-local sample s: the law of the Hogwild kernels
 __device__ __forceinline__ void det_draw(const BprParams& p, int64_t s_local, int32_t& u, int32_t& i, int32_t& j)
 {
-    const uint64_t s = p.sample_base + (uint64_t)s_local;
-    const Philox4 r = philox4x32_10((uint32_t)s, (uint32_t)(s >> 32), p.epoch_lo, p.epoch_hi, p.seed_lo, p.seed_hi);
-    int64_t i_lo, i_len, j_lo, j_len;
-    law_ranges(p.law, s, i_lo, i_len, j_lo, j_len);
-    const int64_t ii = i_lo + (int64_t)range64(r.x, r.y, (uint64_t)i_len);
-    j = p.neg_weighted ? __ldg(p.pairs + range64(r.z, r.w, (uint64_t)p.nnz)).y
-                       : (int32_t)(j_lo + (int64_t)range64(r.z, r.w, (uint64_t)j_len));
+    int64_t ii;
+    draw_sample(p, s_local, ii, j);
     const int2 pr = __ldg(p.pairs + ii);
     u = pr.x;
     i = pr.y;
@@ -1153,18 +867,8 @@ __global__ void __launch_bounds__(256) bpr_det_grad_kernel(const BprParams p, co
         int32_t u, i, j;
         det_draw(p, s_loc, u, i, j);
         // has_non_zero(u, j)  (recom_bpr.pyx:241-243) = key (u, j) in the table
-        const uint64_t key = ((uint64_t)(uint32_t)u << 32) | (uint32_t)j;
-        uint64_t bb = mix64(key) & p.bucket_mask;
-        bool hit = false;
-        for (;;) {
-            const unsigned long long sl = (lane < 4) ? __ldg(p.table + 4 * bb + lane) : 0ull;
-            const unsigned h = __ballot_sync(0xffffffffu, lane < 4 && sl == key);
-            const unsigned f = __ballot_sync(0xffffffffu, lane == 3 && sl != TABLE_EMPTY);
-            if (h) { hit = true; break; }
-            if (!f) break;
-            bb = (bb + 1) & p.bucket_mask;
-        }
-        if (hit) {
+        const uint64_t key = pair_key(u, j);
+        if (group_has<32>(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask, lane)) {
             n_skipped = 1;
         } else {
             const size_t k = (size_t)p.k;
@@ -1358,8 +1062,6 @@ extern "C" int b200_bpr_epoch(const int32_t* pairs, const uint64_t* table, int64
             if (!(flags & B200_SGD_UNBOUNDED) && cap < p.max_groups) p.max_groups = cap;
         }
     }
-    p.debug_skip = 0;
-    if (const char* e = getenv("B200_BPR_DEBUG_SKIP")) p.debug_skip = atoi(e);
     p.U = U; p.V = V; p.B = B; p.k = k; p.lr = lr; p.reg = reg; p.use_bias = use_bias;
     if (p.hinge) p.use_bias = 1;          // MMMF always trains the item biases (recom_mmmf.pyx:149-152)
     p.seed_lo = (uint32_t)seed; p.seed_hi = (uint32_t)(seed >> 32);
@@ -1383,22 +1085,18 @@ extern "C" int b200_bpr_epoch(const int32_t* pairs, const uint64_t* table, int64
 
 static int bpr_replay_launch(ReplayParams& p, int64_t n_users, int64_t n_items, cudaStream_t st)
 {
-    const char* mode = getenv("B200_REPLAY_SERIAL");          // dev knob: 1 = strictly serial warp, 2 = 32-sample windows
+    const char* mode = getenv("B200_REPLAY_SERIAL");          // dev knob: 1 = the strictly serial reference kernel
     ::b200::count_launch();
     if (mode && mode[0] == '1') { bpr_replay_kernel<<<1, 32, 0, st>>>(p); B200_CUDA(cudaGetLastError()); return B200_OK; }
-    if (mode && mode[0] == '2') { bpr_replay_window_kernel<<<1, 1024, 0, st>>>(p); B200_CUDA(cudaGetLastError()); return B200_OK; }
     const size_t fixed = (sizeof(SchedShared) + 15) & ~(size_t)15;
     size_t model = 0;
     if (n_users > 0 && n_items > 0) model = ((size_t)(n_users + n_items) * p.k + (size_t)n_items) * sizeof(float);
     const size_t limit = 227 * 1024 - 1024;
-    if (model > 0 && fixed + model <= limit && !(mode && mode[0] == '3')) {      // 3 = scheduled kernel on the global factors
-        const size_t smem = fixed + model;
-        B200_CUDA(cudaFuncSetAttribute(bpr_replay_sched_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        bpr_replay_sched_kernel<true><<<1, 1024, smem, st>>>(p, n_users, n_items);
-    } else {
-        B200_CUDA(cudaFuncSetAttribute(bpr_replay_sched_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fixed));
-        bpr_replay_sched_kernel<false><<<1, 1024, fixed, st>>>(p, 0, 0);
-    }
+    const bool on_chip = model > 0 && fixed + model <= limit;
+    auto kern = on_chip ? bpr_replay_sched_kernel<true> : bpr_replay_sched_kernel<false>;
+    const size_t smem = on_chip ? fixed + model : fixed;
+    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<1, 1024, smem, st>>>(p, on_chip ? n_users : 0, on_chip ? n_items : 0);
     B200_CUDA(cudaGetLastError());
     return B200_OK;
 }

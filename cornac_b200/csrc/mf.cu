@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(32) mf_replay_kernel(const MfParams<IdT> p)
     if (lane == 0) *p.loss = loss;
 }
 
-// Ordered mode, windowed (same idea as bpr_replay_window_kernel): 32 consecutive ratings are resolved at a
+// Ordered mode, windowed: 32 consecutive ratings are resolved at a
 // time, one per warp, and applied as soon as no EARLIER pending rating of the window has the same user or
 // the same item.  Ratings that share neither commute exactly; the per-epoch loss is summed in rating order
 // afterwards from the per-rating squared errors so that it matches the reference's f32 accumulator.

@@ -3,7 +3,7 @@
 A sample (u, i, j) must see every earlier update of its three rows; samples that share no row commute exactly.  The
 dependency level of a sample = 1 + the largest level among earlier samples that touch one of its rows; all samples of
 one level are independent, and the number of levels is the length of the critical path = the number of sequential steps
-ANY exact schedule needs.  The windowed replay kernel (bpr_replay_window_kernel) resolves this inside windows of 32
+ANY exact schedule needs.  The scheduled replay kernel (bpr_replay_sched_kernel) resolves this inside phases of 1024
 samples; this script measures what window sizes up to the whole epoch would allow.  Pure numpy + the host sampler of libb200cornac.so; no GPU."""
 import os
 import sys
