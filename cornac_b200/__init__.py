@@ -8,7 +8,7 @@ Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b
 plug-ins).  The plug-in classes need the `cornac` package importable (they subclass its
 Recommender so that cornac.Experiment accepts them); the engine does not.
 """
-__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "engine", "B200Error"]
+__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "engine", "B200Error"]
 
 from ._lib import B200Error  # noqa: F401
 
@@ -35,6 +35,9 @@ def __getattr__(name):
     if name == "WMF":
         from .recom_wmf import WMF
         return WMF
+    if name in ("UserKNN", "ItemKNN"):
+        from . import recom_knn
+        return getattr(recom_knn, name)
     if name == "BaselineOnly":
         from .recom_bo import BaselineOnly
         return BaselineOnly

@@ -53,6 +53,13 @@ SIGNATURES = {
                              _c.c_uint, _vp, _vp]),
     "b200_wmf_step": (_int, [_vp, _vp, _vp, _vp, _int, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp,
                              _f32, _f32, _f32, _f32, _f32, _f32, _f32, _f32, _vp, _vp, _vp, _vp]),
+    "b200_knn_similarity_workspace_bytes": (_i64, [_i64]),
+    "b200_knn_similarity": (_int, [_i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _c.c_double, _vp, _vp, _vp]),
+    "b200_knn_row_nnz": (_int, [_i64, _vp, _vp, _vp]),
+    "b200_knn_compact": (_int, [_i64, _vp, _vp, _vp, _vp, _vp]),
+    "b200_knn_score_workspace_bytes": (_i64, [_i64, _i64, _int]),
+    "b200_knn_score_items": (_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
+    "b200_knn_score_users": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),

@@ -7,8 +7,10 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     mf_epoch                       <-> backend_cpu.fit_sgd   (cornac/models/mf/backend_cpu.pyx:58-83)
     score_batch                    <-> fast_dot              (cornac/utils/fast_dot.pyx:40-43)
     topk_rows / rank_topk          <-> Recommender.rank      (cornac/models/recommender.py:476-530)
+    knn_similarity / knn_score     <-> compute_similarity / compute_score (cornac/models/knn/similarity.pyx)
 """
 import numpy as np
+import scipy.sparse as _sp
 import torch
 
 from . import _lib
@@ -443,6 +445,119 @@ class WmfTrainer:
 
     def download(self):
         return self.U.cpu().numpy(), self.V.cpu().numpy()
+
+
+def _csr_arrays(m, what):
+    """int32 indptr / indices and f64 data of a scipy CSR matrix (copies only where the dtype differs)."""
+    if m.nnz >= 2 ** 31:
+        raise B200Error("%s: nnz >= 2^31 is not supported (int32 CSR offsets)" % what)
+    return (np.ascontiguousarray(m.indptr, dtype=np.int32), np.ascontiguousarray(m.indices, dtype=np.int32),
+            np.ascontiguousarray(m.data, dtype=np.float64))
+
+
+def _upload_csr(m, what):
+    ip, ix, dt = _csr_arrays(m, what)
+    if len(ix) == 0:
+        ix, dt = np.zeros(1, np.int32), np.zeros(1)
+    return to_device(ip, torch.int32), to_device(ix, torch.int32), to_device(dt, torch.float64)
+
+
+def knn_similarity(weight, amplify=1.0):
+    """compute_similarity + the amplify map (cornac/models/knn/similarity.pyx:51-105, recom_knn.py:48-55) of the rows of
+    the scipy CSR weight matrix.  Returns (S, sim_mat): the dense symmetric f64 [n, n] device similarity and the same
+    matrix as a host scipy CSR (f64, zeros dropped).  Refuses before allocating when S does not fit the free device memory."""
+    L = require_cuda()
+    weight = weight.tocsr()
+    n, n_cols = (int(x) for x in weight.shape)
+    ws_bytes = int(L.b200_knn_similarity_workspace_bytes(n))
+    need = n * n * 8
+    free, _ = torch.cuda.mem_get_info()
+    if need + ws_bytes > free:
+        raise B200Error("the dense %d x %d f64 similarity needs %d bytes (+ %d bytes of workspace); the device has %d bytes free"
+                        % (n, n, need, ws_bytes, free))
+    cols = weight.T.tocsr()
+    cols.sort_indices()
+    ip, ix, _ = _csr_arrays(weight, "weight matrix")
+    # rows in decreasing work (sum of the lengths of the columns a row touches), so the longest rows start first
+    work = np.zeros(n, dtype=np.int64)
+    if len(ix):
+        np.add.at(work, np.repeat(np.arange(n), np.diff(ip)), np.diff(cols.indptr)[ix])
+    order = np.argsort(-work, kind="stable").astype(np.int32)
+    r_p, r_i, r_d = _upload_csr(weight, "weight matrix")
+    c_p, c_i, c_d = _upload_csr(cols, "weight matrix")
+    ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device="cuda")
+    S = torch.empty((n, n), dtype=torch.float64, device="cuda")
+    st = current_stream()
+    check(L.b200_knn_similarity(n, ptr(r_p), ptr(r_i), ptr(r_d), n_cols, ptr(c_p), ptr(c_i), ptr(c_d),
+                                ptr(to_device(order, torch.int32)), float(amplify), ptr(ws) if ws_bytes else None, ptr(S), st),
+          "b200_knn_similarity")
+    del ws
+    counts = torch.empty(n, dtype=torch.int32, device="cuda")
+    check(L.b200_knn_row_nnz(n, ptr(S), ptr(counts), st), "b200_knn_row_nnz")
+    indptr = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(counts.cpu().numpy(), out=indptr[1:])
+    nnz = int(indptr[-1])
+    if nnz >= 2 ** 31:
+        raise B200Error("the similarity has %d non-zeros: nnz >= 2^31 is not supported (int32 CSR offsets)" % nnz)
+    d_ptr = to_device(indptr, torch.int32)
+    d_idx = torch.empty(max(nnz, 1), dtype=torch.int32, device="cuda")
+    d_val = torch.empty(max(nnz, 1), dtype=torch.float64, device="cuda")
+    check(L.b200_knn_compact(n, ptr(S), ptr(d_ptr), ptr(d_idx), ptr(d_val), st), "b200_knn_compact")
+    sim = _sp.csr_matrix((d_val[:nnz].cpu().numpy(), d_idx[:nnz].cpu().numpy(), indptr.astype(np.int32)), shape=(n, n))
+    return S, sim
+
+
+def knn_dense(sim):
+    """The dense f64 device matrix of a host scipy CSR similarity (after load(): the device state is not pickled)."""
+    require_cuda()
+    n = int(sim.shape[0])
+    need = n * n * 8
+    free, _ = torch.cuda.mem_get_info()
+    if need > free:
+        raise B200Error("the dense %d x %d f64 similarity needs %d bytes; the device has %d bytes free" % (n, n, need, free))
+    coo = sim.tocoo()
+    S = torch.zeros((n, n), dtype=torch.float64, device="cuda")
+    S.view(-1)[to_device(coo.row.astype(np.int64) * n + coo.col, torch.int64)] = to_device(coo.data, torch.float64)
+    return S
+
+
+class KnnRatings:
+    """Device copy of the CSR rating matrix the scores read: the user-item matrix (ItemKNN) or the item-user matrix
+    (UserKNN), and the users' mean ratings."""
+
+    def __init__(self, m, mean):
+        require_cuda()
+        m = m.tocsr().copy()
+        m.sort_indices()                             # the candidates are visited in descending neighbour index
+        self.n_rows, self.n_cols = (int(x) for x in m.shape)
+        self.indptr, self.indices, self.data = _upload_csr(m, "rating matrix")
+        self.mean = to_device(np.asarray(mean, dtype=np.float64), torch.float64)
+
+
+def knn_score(user_mode, S, users, ratings, k):
+    """compute_score (cornac/models/knn/similarity.pyx:154-201) plus the user's mean for each user of `users`:
+    f64 [n_q, n_items] device scores.  user_mode: UserKNN (S is [n_users, n_users], ratings the item-user matrix);
+    otherwise ItemKNN (S is [n_items, n_items], ratings the user-item matrix)."""
+    L = require_cuda()
+    _dev(S, torch.float64, "S")
+    if k < 1:
+        raise B200Error("k must be >= 1, got %d" % k)
+    users = users if isinstance(users, torch.Tensor) else to_device(np.asarray(users, dtype=np.int64), torch.int64)
+    _dev(users, torch.int64, "users")
+    n_q = int(users.numel())
+    n_users = int(S.shape[0]) if user_mode else ratings.n_rows
+    n_items = ratings.n_rows if user_mode else int(S.shape[0])
+    out = torch.empty((n_q, n_items), dtype=torch.float64, device="cuda")
+    ws_bytes = int(L.b200_knn_score_workspace_bytes(n_q, n_users if user_mode else 0, int(k)))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda") if ws_bytes else None
+    if user_mode:
+        rc = L.b200_knn_score_users(ptr(users), n_q, n_users, n_items, ptr(ratings.indptr), ptr(ratings.indices),
+                                    ptr(ratings.data), ptr(S), ptr(ratings.mean), int(k), ptr(ws), ptr(out), current_stream())
+    else:
+        rc = L.b200_knn_score_items(ptr(users), n_q, n_items, ptr(ratings.indptr), ptr(ratings.indices), ptr(ratings.data),
+                                    ptr(S), ptr(ratings.mean), int(k), ptr(ws), ptr(out), current_stream())
+    check(rc, "b200_knn_score_users" if user_mode else "b200_knn_score_items")
+    return out
 
 
 def score_batch(U, V, user_idx=None, item_base=None, user_off=None, n_items=None, out=None):

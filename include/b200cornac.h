@@ -225,6 +225,46 @@ B200_API int b200_wmf_step(const int32_t* csc_indptr, const int32_t* csc_rows, c
                            int32_t* slot_of, float* gV_scratch, double* loss, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Neighbourhood models (UserKNN / ItemKNN, cornac/models/knn).  CSR inputs are int32 indptr / indices with f64 data.
+ *
+ * Replaces compute_similarity (cornac/models/knn/similarity.pyx:51-105) followed by the amplify map of recom_knn.py:48-55:
+ * out = the dense symmetric f64 [n, n] cosine similarity of the n rows of the weight matrix, bit-identical to the compiled
+ * reference for amplify == 1 (ordered sums, every product and sum rounded, denominator sqrt(D1 * D2)).
+ *   row_*      the weight matrix (n rows, n_cols columns), entries of a row in the order the reference visits them
+ *   col_*      its transpose (n_cols rows), indices ascending within each row
+ *   order      device int32[n], a permutation of the rows (the order the CTAs take them in; heaviest first)
+ *   amplify    w -> sign(w) |w|^amplify on every non-zero similarity (1 = none)
+ *   workspace  device scratch of b200_knn_similarity_workspace_bytes(n) bytes (0 = none needed, may be NULL)        */
+B200_API int64_t b200_knn_similarity_workspace_bytes(int64_t n);
+B200_API int b200_knn_similarity(int64_t n, const int32_t* row_indptr, const int32_t* row_indices, const double* row_data,
+                                 int64_t n_cols, const int32_t* col_indptr, const int32_t* col_indices, const double* col_data,
+                                 const int32_t* order, double amplify, void* workspace, double* out, void* stream);
+
+/* The csr_matrix(sim_mat) step of compute_similarity (similarity.pyx:102) in two passes: counts[r] = non-zeros of row r of
+ * the dense [n, n] matrix; the caller turns the counts into indptr (int32 [n+1]) and b200_knn_compact writes the column
+ * indices (ascending) and values of every row.                                                                           */
+B200_API int b200_knn_row_nnz(int64_t n, const double* sim, int32_t* counts, void* stream);
+B200_API int b200_knn_compact(int64_t n, const double* sim, const int32_t* indptr, int32_t* indices, double* data, void* stream);
+
+/* Replaces compute_score (similarity.pyx:154-201, SparseNeighbors / TopK of similarity.h:15-89) for a batch of users:
+ * out[q, i] = mean[users[q]] + sum(w v) / (sum |w| + 1e-8) over the k neighbours the reference keeps (candidates in
+ * descending neighbour index; after the first k, one is kept only if its weight is strictly greater than the smallest kept
+ * weight, and it replaces the smallest kept (weight, value) pair).  out is device f64 [n_q, n_items].
+ *   b200_knn_score_items (ItemKNN.score): ui_* = the user-item matrix, sim = dense [n_items, n_items]; candidates of (u, i)
+ *     are the items j with ui[u,j] != 0 and sim[i,j] != 0, weight sim[i,j], value ui[u,j].
+ *   b200_knn_score_users (UserKNN.score): iu_* = the item-user matrix, sim = dense [n_users, n_users]; candidates of (u, i)
+ *     are the users v in row i of iu with sim[u,v] != 0, weight sim[u,v], value iu[i,v].
+ *   workspace  device scratch of b200_knn_score_workspace_bytes(n_q, n_stage, k) bytes, n_stage = n_users for
+ *              b200_knn_score_users and 0 for b200_knn_score_items (0 bytes = none needed, may be NULL)              */
+B200_API int64_t b200_knn_score_workspace_bytes(int64_t n_q, int64_t n_stage, int k);
+B200_API int b200_knn_score_items(const int64_t* users, int64_t n_q, int64_t n_items, const int32_t* ui_indptr,
+                                  const int32_t* ui_indices, const double* ui_data, const double* sim, const double* mean,
+                                  int k, void* workspace, double* out, void* stream);
+B200_API int b200_knn_score_users(const int64_t* users, int64_t n_q, int64_t n_users, int64_t n_items,
+                                  const int32_t* iu_indptr, const int32_t* iu_indices, const double* iu_data,
+                                  const double* sim, const double* mean, int k, void* workspace, double* out, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
