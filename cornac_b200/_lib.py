@@ -60,9 +60,15 @@ SIGNATURES = {
     "b200_knn_score_workspace_bytes": (_i64, [_i64, _i64, _int]),
     "b200_knn_score_items": (_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
     "b200_knn_score_users": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
+    "b200_pmf_schedule": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
+    "b200_pmf_fit": (_int, [_int, _vp, _vp, _vp, _vp, _i32, _i64, _int, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _vp,
+                            _vp, _vp]),
+    "b200_pmf_sigmoid": (_int, [_vp, _i64, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),
+    "b200_score_batch_f64": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp]),
+    "b200_topk_rows_f64": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),
     "b200_rank_topk_workspace_bytes": (_i64, [_i64, _i64, _int, _int]),
     "b200_rank_topk": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp, _int, _vp, _vp,
                               _vp, _i64, _vp]),
@@ -89,6 +95,7 @@ BPR_NEG_WEIGHTED = 8
 BPR_LOSS_HINGE = 16
 BPR_BLOCKED = 32
 BPR_DETERMINISTIC = 64
+PMF_LINEAR, PMF_NON_LINEAR = 0, 1
 METRIC_NDCG, METRIC_PRECISION, METRIC_RECALL, METRIC_FMEASURE, METRIC_HIT, METRIC_NCRR = range(6)
 
 _lib = None

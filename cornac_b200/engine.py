@@ -8,6 +8,8 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     score_batch                    <-> fast_dot              (cornac/utils/fast_dot.pyx:40-43)
     topk_rows / rank_topk          <-> Recommender.rank      (cornac/models/recommender.py:476-530)
     knn_similarity / knn_score     <-> compute_similarity / compute_score (cornac/models/knn/similarity.pyx)
+    pmf_schedule / pmf_fit         <-> pmf_linear / pmf_non_linear (cornac/models/pmf/cython/pmf.pyx:55-173)
+    score_batch_f64 / topk_rows_f64 <-> PMF.score / Recommender.rank (cornac/models/pmf/recom_pmf.py:191-222)
 """
 import numpy as np
 import scipy.sparse as _sp
@@ -588,6 +590,101 @@ def topk_rows(scores, topk, excl_indptr=None, excl_indices=None):
     check(L.b200_topk_rows(ptr(scores), n_q, n_items, ptr(excl_indptr), ptr(excl_indices), int(topk), ptr(ids),
                            ptr(sc), current_stream()), "b200_topk_rows")
     return ids, sc
+
+
+def score_batch_f64(U, V, user_idx=None, n_items=None, out=None):
+    """out[q, i] = sum_f U[user_idx[q], f] * V[i, f] in f64 (f ascending, no FMA) for i < n_items."""
+    L = require_cuda()
+    _dev(U, torch.float64, "U"), _dev(V, torch.float64, "V")
+    n_items = V.shape[0] if n_items is None else int(n_items)
+    n_q = U.shape[0] if user_idx is None else user_idx.numel()
+    if user_idx is not None:
+        _dev(user_idx, torch.int64, "user_idx")
+    if out is None:
+        out = torch.empty((n_q, n_items), dtype=torch.float64, device=U.device)
+    check(L.b200_score_batch_f64(ptr(U), ptr(user_idx), n_q, ptr(V), n_items, int(V.shape[1]),
+                                 ptr(_dev(out, torch.float64, "out")), current_stream()), "b200_score_batch_f64")
+    return out
+
+
+def topk_rows_f64(scores, topk, excl_indptr=None, excl_indices=None):
+    """topk_rows over f64 score rows: exact top-k (score desc, id asc) with per-row exclusions."""
+    L = require_cuda()
+    _dev(scores, torch.float64, "scores")
+    n_q, n_items = scores.shape
+    ids = torch.empty((n_q, topk), dtype=torch.int32, device=scores.device)
+    sc = torch.empty((n_q, topk), dtype=torch.float64, device=scores.device)
+    if excl_indptr is not None:
+        _dev(excl_indptr, torch.int64, "excl_indptr"), _dev(excl_indices, torch.int32, "excl_indices")
+    check(L.b200_topk_rows_f64(ptr(scores), n_q, n_items, ptr(excl_indptr), ptr(excl_indices), int(topk), ptr(ids),
+                               ptr(sc), current_stream()), "b200_topk_rows_f64")
+    return ids, sc
+
+
+def pmf_schedule(uid, iid, n_users, n_items):
+    """Level schedule of PMF's ratings (host, no device needed): (order int32 [nnz], level_ptr int32 [n_levels + 1]).
+    Slot s of the schedule is stored rating order[s]; level l is slots [level_ptr[l], level_ptr[l+1]), its ratings touch
+    pairwise disjoint user and item rows, and inside a level the slots keep the stored order."""
+    L = _lib.load()
+    uid = np.ascontiguousarray(uid, dtype=np.int32)
+    iid = np.ascontiguousarray(iid, dtype=np.int32)
+    nnz = len(uid)
+    if len(iid) != nnz:
+        raise B200Error("uid and iid differ in length (%d, %d)" % (nnz, len(iid)))
+    order = np.empty(nnz, dtype=np.int32)
+    level_ptr = np.empty(nnz + 1, dtype=np.int32)
+    n_levels = np.zeros(1, dtype=np.int32)
+    check(L.b200_pmf_schedule(ptr(uid), ptr(iid), nnz, int(n_users), int(n_items), ptr(order), ptr(level_ptr),
+                              ptr(n_levels)), "b200_pmf_schedule")
+    return order, level_ptr[: int(n_levels[0]) + 1].copy()
+
+
+class PmfData:
+    """Device copy of PMF's ratings in schedule order (b200_pmf_schedule), built once per fit and used by every epoch."""
+
+    def __init__(self, uid, iid, rat, n_users, n_items):
+        require_cuda()
+        self.nnz = len(uid)
+        self.order_host, level_ptr = pmf_schedule(uid, iid, n_users, n_items)
+        self.n_levels = len(level_ptr) - 1
+        o = self.order_host
+        self.uid = to_device(np.asarray(uid, dtype=np.int32)[o], torch.int32)
+        self.iid = to_device(np.asarray(iid, dtype=np.int32)[o], torch.int32)
+        self.rat = to_device(np.asarray(rat, dtype=np.float32)[o], torch.float32)
+        self.level_ptr = to_device(level_ptr, torch.int32)
+        self.order = to_device(o, torch.int32)
+
+
+def pmf_fit(data, variant, U, V, cache_u, cache_v, n_epochs, lambda_reg, learning_rate, gamma, loss=None):
+    """n_epochs epochs of pmf_linear / pmf_non_linear (pmf.pyx:55-173) over `data` (PmfData), updating the f64 device
+    tensors U, V, cache_u, cache_v in place.  loss: optional f64 device tensor [n_epochs, nnz] that receives each rating's
+    loss term at its stored index."""
+    L = require_cuda()
+    variants = {"linear": _lib.PMF_LINEAR, "non_linear": _lib.PMF_NON_LINEAR}
+    if variant not in variants:
+        raise B200Error('variant must be one of {"linear","non_linear"}, got %r' % (variant,))
+    k = int(U.shape[1])
+    for t, name in ((U, "U"), (V, "V"), (cache_u, "cache_u"), (cache_v, "cache_v")):
+        _dev(t, torch.float64, name)
+        if t.dim() != 2 or int(t.shape[1]) != k:
+            raise B200Error("%s must be 2-D with %d columns" % (name, k))
+    if loss is not None:
+        _dev(loss, torch.float64, "loss")
+        if loss.numel() != int(n_epochs) * data.nnz:
+            raise B200Error("loss must hold n_epochs * nnz = %d values" % (int(n_epochs) * data.nnz))
+    check(L.b200_pmf_fit(variants[variant], ptr(data.uid), ptr(data.iid), ptr(data.rat), ptr(data.level_ptr),
+                         data.n_levels, data.nnz, k, ptr(U), ptr(V), ptr(cache_u), ptr(cache_v), int(n_epochs),
+                         float(lambda_reg), float(learning_rate), float(gamma), ptr(loss),
+                         ptr(data.order) if loss is not None else None, current_stream()), "b200_pmf_fit")
+
+
+def pmf_sigmoid(z):
+    """The reference PMF sigmoid (pmf.pyx:27-37, expf in f32) of a f32 device tensor, as b200_pmf_fit evaluates it."""
+    L = require_cuda()
+    _dev(z, torch.float32, "z")
+    out = torch.empty_like(z)
+    check(L.b200_pmf_sigmoid(ptr(z), z.numel(), ptr(out), current_stream()), "b200_pmf_sigmoid")
+    return out
 
 
 def rank_pack_items(V, item_base=None, n_items=None):

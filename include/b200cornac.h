@@ -265,6 +265,42 @@ B200_API int b200_knn_score_users(const int64_t* users, int64_t n_q, int64_t n_u
                                   const double* sim, const double* mean, int k, void* workspace, double* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * PMF (cornac/models/pmf/cython/pmf.pyx:55-173: pmf_linear / pmf_non_linear), SGD with RMSProp over the ratings in
+ * stored order, in f64.  Rating r must see every earlier update of its user row and of its item row; two ratings that
+ * share no row commute exactly.  level(r) = 1 + max(level of the previous rating of the same user, level of the previous
+ * rating of the same item): the ratings of one level touch pairwise disjoint rows, so applying the levels in turn, in
+ * any order inside a level, gives the serial loop's result bit for bit.
+ *
+ * b200_pmf_schedule (HOST): the level schedule of the ratings (uid, iid: host int32[nnz], stored order).
+ *   order       host int32[nnz]: the stored index of each scheduled slot, level-major, stored order inside a level
+ *   level_ptr   host int32[nnz + 1] (capacity): level l is slots [level_ptr[l], level_ptr[l+1])
+ *   n_levels    host int32: number of levels (0 when nnz == 0)
+ *
+ * b200_pmf_fit: n_epochs epochs of pmf_linear (variant B200_PMF_LINEAR) or pmf_non_linear (B200_PMF_NON_LINEAR) in one
+ * launch (one CTA walking the levels, a barrier between consecutive levels).
+ *   uid, iid, rat   device int32 / int32 / f32 [nnz], already permuted into schedule order (x[order[slot]])
+ *   level_ptr       device int32[n_levels + 1]
+ *   U, V            device f64 [n_users, k] / [n_items, k], updated in place
+ *   cache_u/v       device f64, same shapes: the RMSProp caches (zero at the start of a fit, kept across calls)
+ *   lambda_reg, learning_rate, gamma   f32, as the reference's C `float` parameters (used in f64 expressions)
+ *   loss            device f64 [n_epochs, nnz] or NULL: loss[e, order[slot]] = e*e + lambda_reg*(|U[u]|^2 + |V[i]|^2)
+ *                   of that rating in epoch e; summing a row in stored order gives the reference's loss[epoch]
+ *   order           device int32[nnz]; read only when loss != NULL
+ * Calling it twice with n_epochs = a and b is the same as calling it once with a + b.
+ *
+ * b200_pmf_sigmoid: out[j] = the reference's sigmoid(z[j]) (pmf.pyx:27-37; C++ resolves exp(float) to expf) as the
+ * fit kernel evaluates it, for device f32 z / out [n].                                                                  */
+#define B200_PMF_LINEAR 0
+#define B200_PMF_NON_LINEAR 1
+B200_API int b200_pmf_schedule(const int32_t* uid, const int32_t* iid, int64_t nnz, int64_t n_users, int64_t n_items,
+                               int32_t* order, int32_t* level_ptr, int32_t* n_levels);
+B200_API int b200_pmf_fit(int variant, const int32_t* uid, const int32_t* iid, const float* rat, const int32_t* level_ptr,
+                          int32_t n_levels, int64_t nnz, int k, double* U, double* V, double* cache_u, double* cache_v,
+                          int n_epochs, float lambda_reg, float learning_rate, float gamma, double* loss,
+                          const int32_t* order, void* stream);
+B200_API int b200_pmf_sigmoid(const float* z, int64_t n, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
@@ -290,6 +326,19 @@ B200_API int b200_score(const float* U, int64_t user_idx, const float* V, int64_
 B200_API int b200_topk_rows(const float* scores, int64_t n_q, int64_t n_items,
                             const int64_t* excl_indptr, const int32_t* excl_indices,
                             int topk, int32_t* out_ids, float* out_scores, void* stream);
+
+/* f64 scores of a batch of users, as PMF.score(u) defines them (cornac/models/pmf/recom_pmf.py:215-216, V.dot(U[u])):
+ *   out[q, i] = sum_f U[user_idx[q], f] * V[i, f]   in f64, f ascending, every product and every sum rounded on its own
+ *   (no FMA), so the result is a fixed function of the inputs.
+ *   user_idx device int64[n_q] (NULL = rows 0..n_q-1 of U); out device f64[n_q, n_items]                               */
+B200_API int b200_score_batch_f64(const double* U, const int64_t* user_idx, int64_t n_q, const double* V, int64_t n_items,
+                                  int k, double* out, void* stream);
+
+/* b200_topk_rows over f64 score rows: the same exclusion-aware radix select (over 64-bit keys) and the same total order
+ * (score desc, id asc).  Rows must be NaN-free.  out_scores device f64[n_q, topk].                                      */
+B200_API int b200_topk_rows_f64(const double* scores, int64_t n_q, int64_t n_items,
+                                const int64_t* excl_indptr, const int32_t* excl_indices,
+                                int topk, int32_t* out_ids, double* out_scores, void* stream);
 
 /* Fused rank: scores (as b200_score_batch) + exclusion + top-k (as b200_topk_rows) for a
  * batch of users without materialising the [n_q, n_items] score matrix.  Tensor-core
