@@ -1,6 +1,6 @@
 """cornac_b200 -- H100 (sm_90a) implementation of Cornac's BPR / MF train-and-rank hot path.
 
-    from cornac_b200 import BPR, MF, PMF   # drop-in for cornac.models.BPR / MF / PMF
+    from cornac_b200 import BPR, MF, PMF, NMF   # drop-in for cornac.models.BPR / MF / PMF / NMF
     cornac.Experiment(eval_method=..., models=[BPR(k=64, ...)], metrics=[...]).run()
 
 Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b200.engine
@@ -8,7 +8,7 @@ Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b
 plug-ins).  The plug-in classes need the `cornac` package importable (they subclass its
 Recommender so that cornac.Experiment accepts them); the engine does not.
 """
-__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "engine", "B200Error"]
+__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "engine", "B200Error"]
 
 from ._lib import B200Error  # noqa: F401
 
@@ -41,6 +41,9 @@ def __getattr__(name):
     if name == "PMF":
         from .recom_pmf import PMF
         return PMF
+    if name == "NMF":
+        from .recom_nmf import NMF
+        return NMF
     if name == "BaselineOnly":
         from .recom_bo import BaselineOnly
         return BaselineOnly

@@ -64,6 +64,9 @@ SIGNATURES = {
     "b200_pmf_fit": (_int, [_int, _vp, _vp, _vp, _vp, _i32, _i64, _int, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _vp,
                             _vp, _vp]),
     "b200_pmf_sigmoid": (_int, [_vp, _i64, _vp, _vp]),
+    "b200_nmf_prepare": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
+    "b200_nmf_fit": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _int,
+                            _vp, _vp, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _f32, _f32, _f32, _int, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),

@@ -10,6 +10,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     knn_similarity / knn_score     <-> compute_similarity / compute_score (cornac/models/knn/similarity.pyx)
     pmf_schedule / pmf_fit         <-> pmf_linear / pmf_non_linear (cornac/models/pmf/cython/pmf.pyx:55-173)
     score_batch_f64 / topk_rows_f64 <-> PMF.score / Recommender.rank (cornac/models/pmf/recom_pmf.py:191-222)
+    nmf_prepare / nmf_fit          <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
 """
 import numpy as np
 import scipy.sparse as _sp
@@ -685,6 +686,97 @@ def pmf_sigmoid(z):
     out = torch.empty_like(z)
     check(L.b200_pmf_sigmoid(ptr(z), z.numel(), ptr(out), current_stream()), "b200_pmf_sigmoid")
     return out
+
+
+def nmf_prepare(indptr, indices, n_items):
+    """Host checks of the CSR ratings and NMF's stable CSC position map (b200_nmf_prepare, no device needed):
+    (csc_ptr int32 [n_items + 1], csc_pos int32 [nnz], item_order int32 [n_items]).  Column i lists the stored indices of
+    item i's ratings in stored order; item_order is the items by decreasing number of ratings."""
+    L = _lib.load()
+    indptr = np.ascontiguousarray(indptr, dtype=np.int32)
+    indices = np.ascontiguousarray(indices, dtype=np.int32)
+    nnz = len(indices)
+    csc_ptr = np.empty(int(n_items) + 1, dtype=np.int32)
+    csc_pos = np.empty(nnz, dtype=np.int32)
+    item_order = np.empty(int(n_items), dtype=np.int32)
+    check(L.b200_nmf_prepare(ptr(indptr), ptr(indices), len(indptr) - 1, int(n_items), nnz, ptr(csc_ptr), ptr(csc_pos),
+                             ptr(item_order)), "b200_nmf_prepare")
+    return csc_ptr, csc_pos, item_order
+
+
+class NmfData:
+    """Device copy of NMF's ratings, built once per fit and used by every epoch: the CSR (indptr, indices, f32 ratings),
+    its stable CSC transpose (b200_nmf_prepare) and, only when the biases are trained, the ratings in the level order of
+    b200_pmf_schedule."""
+
+    def __init__(self, indptr, indices, rating, n_items, use_bias):
+        require_cuda()
+        if len(indices) >= 2 ** 31:
+            raise B200Error("nnz >= 2^31 is not supported (int32 CSR offsets)")
+        indptr = np.ascontiguousarray(indptr, dtype=np.int32)
+        indices = np.ascontiguousarray(indices, dtype=np.int32)
+        rating = np.ascontiguousarray(rating, dtype=np.float32)
+        self.n_users, self.n_items, self.nnz = len(indptr) - 1, int(n_items), len(indices)
+        if len(rating) != self.nnz:
+            raise B200Error("rating has %d values for %d ratings" % (len(rating), self.nnz))
+        csc_ptr, csc_pos, item_order = nmf_prepare(indptr, indices, n_items)
+        uid = np.repeat(np.arange(self.n_users, dtype=np.int32), np.diff(indptr))
+        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
+        self.indptr = to_device(indptr, torch.int32)
+        self.indices = to_device(pad(indices), torch.int32)
+        self.rating = to_device(pad(rating), torch.float32)
+        self.csc_ptr = to_device(csc_ptr, torch.int32)
+        self.csc_pos = to_device(pad(csc_pos), torch.int32)
+        self.csc_row = to_device(pad(uid[csc_pos]), torch.int32)
+        self.csc_val = to_device(pad(rating[csc_pos]), torch.float32)
+        self.item_order = to_device(pad(item_order), torch.int32)
+        self.use_bias = bool(use_bias)
+        self.n_levels = 0
+        self.s_uid = self.s_iid = self.s_rat = self.s_pos = self.level_ptr = None
+        if self.use_bias:
+            order, level_ptr = pmf_schedule(uid, indices, self.n_users, self.n_items)
+            self.n_levels = len(level_ptr) - 1
+            self.s_uid = to_device(pad(uid[order]), torch.int32)
+            self.s_iid = to_device(pad(indices[order]), torch.int32)
+            self.s_rat = to_device(pad(rating[order]), torch.float32)
+            self.s_pos = to_device(pad(order), torch.int32)
+            self.level_ptr = to_device(level_ptr, torch.int32)
+        self.rp = torch.empty(max(self.nnz, 1), dtype=torch.float32, device="cuda")
+
+
+def nmf_fit(data, U, V, Bu, Bi, n_epochs, mu=0.0, learning_rate=0.005, lambda_u=0.06, lambda_v=0.06, lambda_bu=0.02,
+            lambda_bi=0.02, loss=None, workspace=None):
+    """n_epochs epochs of NMF._fit_sgd (recom_nmf.pyx:182-267) over `data` (NmfData), updating the f32 device tensors U,
+    V, Bu, Bi in place, bit for bit as the reference's serial loop.  The biases are trained when data.use_bias; they enter
+    the predictions either way.  The hyperparameters are rounded to f32.  loss: optional f64 device tensor [n_epochs]
+    that receives each epoch's sum err^2 + lambda_u |U|^2 + lambda_v |V|^2 (f64, not the reference's f32 order).
+    workspace: optional f32 device tensor shaped like U (allocated per call otherwise)."""
+    L = require_cuda()
+    k = int(U.shape[1]) if U.dim() == 2 else 0
+    for t, name, rows in ((U, "U", data.n_users), (V, "V", data.n_items)):
+        _dev(t, torch.float32, name)
+        if t.dim() != 2 or int(t.shape[0]) != rows or int(t.shape[1]) != k or k < 1:
+            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, max(k, 1), tuple(t.shape)))
+    for t, name, rows in ((Bu, "Bu", data.n_users), (Bi, "Bi", data.n_items)):
+        _dev(t, torch.float32, name)
+        if t.numel() != rows:
+            raise B200Error("%s must hold %d values, got %d" % (name, rows, t.numel()))
+    if loss is not None:
+        _dev(loss, torch.float64, "loss")
+        if loss.numel() != int(n_epochs):
+            raise B200Error("loss must hold n_epochs = %d values" % int(n_epochs))
+    if workspace is None:
+        workspace = torch.empty_like(U)
+    _dev(workspace, torch.float32, "workspace")
+    if workspace.numel() < U.numel() or workspace.data_ptr() == U.data_ptr():
+        raise B200Error("workspace must hold U.numel() floats and must not alias U")
+    f32 = lambda x: float(np.float32(x))              # noqa: E731
+    check(L.b200_nmf_fit(ptr(data.indptr), ptr(data.indices), ptr(data.rating), data.n_users, data.n_items, data.nnz,
+                         ptr(data.csc_ptr), ptr(data.csc_row), ptr(data.csc_val), ptr(data.csc_pos), ptr(data.item_order),
+                         ptr(data.s_uid), ptr(data.s_iid), ptr(data.s_rat), ptr(data.s_pos), ptr(data.level_ptr),
+                         data.n_levels, k, ptr(U), ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs),
+                         f32(mu), f32(learning_rate), f32(lambda_u), f32(lambda_v), f32(lambda_bu), f32(lambda_bi),
+                         int(data.use_bias), ptr(loss), current_stream()), "b200_nmf_fit")
 
 
 def rank_pack_items(V, item_base=None, n_items=None):

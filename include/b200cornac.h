@@ -301,6 +301,41 @@ B200_API int b200_pmf_fit(int variant, const int32_t* uid, const int32_t* iid, c
 B200_API int b200_pmf_sigmoid(const float* z, int64_t n, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * NMF (cornac/models/nmf/recom_nmf.pyx:182-267), multiplicative updates in plain IEEE f32, bit-identical to the
+ * reference's serial loop.  Per epoch: a pass over the ratings in stored (CSR) order computes each prediction rp and,
+ * with use_bias, steps the biases; then U and V are updated element-wise from ordered sums over each user's row and each
+ * item's column (r * other factor and rp * other factor), the item sums reading the U the epoch started with.
+ *
+ * b200_nmf_prepare (HOST): checks the CSR (indptr int32[n_users + 1], indices int32[nnz]: every item in [0, n_items))
+ * and builds the stable CSC position map:
+ *   csc_ptr     host int32[n_items + 1]: column i is CSC entries [csc_ptr[i], csc_ptr[i+1])
+ *   csc_pos     host int32[nnz]: the stored index of each CSC entry; stored order inside a column
+ *   item_order  host int32[n_items]: items by decreasing number of ratings (ties by id), the order columns are launched in
+ *
+ * b200_nmf_fit: n_epochs epochs; calling it twice with a and b epochs is the same as calling it once with a + b.
+ *   indptr, indices, rating   device CSR int32 / int32 / f32
+ *   csc_ptr, csc_pos, item_order   device copies of b200_nmf_prepare's output
+ *   csc_row, csc_val          device int32 / f32 [nnz]: the user and rating of each CSC entry
+ *   s_uid, s_iid, s_rat, s_pos, level_ptr, n_levels   with use_bias (else NULL / 0): the ratings in the level order of
+ *                             b200_pmf_schedule (applied to the stored order), s_pos = their stored indices
+ *   U, V, Bu, Bi              device f32 [n_users, k] / [n_items, k] / [n_users] / [n_items], updated in place; Bu and
+ *                             Bi enter every prediction and are trained only when use_bias
+ *   rp                        device f32 [nnz] workspace (the predictions of the last epoch on return)
+ *   U_work                    device f32 [n_users, k] workspace, not aliasing U
+ *   mu, learning_rate, lambda_*   f32, as the reference's `floating` locals
+ *   loss                      device f64 [n_epochs] or NULL: += sum err^2 + lambda_u |U|^2 + lambda_v |V|^2 per epoch,
+ *                             summed in f64 in no fixed order (a progress figure; not the reference's f32 sum)      */
+B200_API int b200_nmf_prepare(const int32_t* indptr, const int32_t* indices, int64_t n_users, int64_t n_items, int64_t nnz,
+                              int32_t* csc_ptr, int32_t* csc_pos, int32_t* item_order);
+B200_API int b200_nmf_fit(const int32_t* indptr, const int32_t* indices, const float* rating, int64_t n_users,
+                          int64_t n_items, int64_t nnz, const int32_t* csc_ptr, const int32_t* csc_row, const float* csc_val,
+                          const int32_t* csc_pos, const int32_t* item_order, const int32_t* s_uid, const int32_t* s_iid,
+                          const float* s_rat, const int32_t* s_pos, const int32_t* level_ptr, int32_t n_levels, int k,
+                          float* U, float* V, float* Bu, float* Bi, float* rp, float* U_work, int n_epochs, float mu,
+                          float learning_rate, float lambda_u, float lambda_v, float lambda_bu, float lambda_bi,
+                          int use_bias, double* loss, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
