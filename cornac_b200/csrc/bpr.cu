@@ -14,6 +14,8 @@
 // HBM-bound integer/gather work: no tensor cores here by design (DESIGN.md, K1).
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "sgd_common.cuh"
 
 namespace b200 {
@@ -815,145 +817,291 @@ static int launch_hogwild(const BprParams& p, cudaStream_t st)
 
 // ---------------------------------------------------------------------------------------
 // Deterministic throughput mode (B200_BPR_DETERMINISTIC): the epoch's samples run in rounds of at most DET_ROUND.  Every
-// sample of a round reads the factors as the previous round left them (bpr_det_grad_kernel writes nothing but the
-// accumulators), and the round's updates are summed in 2^-40 fixed point with integer atomics -- exact, so their order
-// does not matter -- before bpr_det_apply_kernel adds each touched element's sum once.  The result depends on the
-// seed and the sample law only, not on thread timing: a run repeats bit for bit.  A round is about as many samples as
-// the Hogwild kernels keep in flight, so the updates of a popular row are summed against a similar staleness.
+// sample of a round reads the factors as the previous round left them, and each element of a row gets ONE update per
+// round, x <- x + (float)(Q 2^-40), where Q is the exact (wrapping int64) sum of the round's 2^-40 fixed-point deltas of
+// that element -- so the order in which the samples run does not matter and a run repeats bit for bit.  A round is about
+// as many samples as the Hogwild kernels keep in flight, so the updates of a popular row are summed against a similar
+// staleness.  Per round r the work is split in three phases, ordered by kernel boundaries on one stream only:
+//   plan   (inside bpr_det_apply_kernel of round r - 1; a prologue launch of the same kernel plans round 0): one thread per
+//          sample draws it, runs the skip test, writes its record {u, i, j, live} and counts the touches of its three rows;
+//          the touch that makes a row SHARED (count 1 -> 2) gives it a slot of a compact accumulator (which row gets which
+//          slot depends on timing, but the sums are exact integers, so it does not change the result);
+//   grad   (bpr_det_grad_kernel): one warp per record computes score, z and the deltas.  A row the sample is the only
+//          toucher of is read by no other sample of the round, so the warp adds its deltas to it at once; the deltas of a
+//          shared row go into the row's slot with integer atomics;
+//   apply  (bpr_det_apply_kernel): one warp per slot adds the slot's sums to its row and clears the slot.
+// A live sample never touches one item row twice (j == i means (u, j) is an interaction: the sample is skipped), so a
+// row touched once receives exactly one term.  The plan state is double-buffered by round parity: the plan of round
+// r + 1 reads only the inputs and writes only the other parity, so it shares nothing with the apply of round r.
 constexpr int64_t DET_ROUND = 16384;
 constexpr double DET_SCALE = 1099511627776.0;       // 2^40
+constexpr unsigned DET_ITEM = 0x80000000u;          // row_of_slot tag of an item row (user rows carry their id alone)
 
-struct DetAcc {
-    unsigned long long* U;      // [n_users * k]  fixed-point sums of the round
-    unsigned long long* V;      // [n_neg * k]
-    unsigned long long* B;      // [n_neg]
+struct DetPlan {
+    int4* rec;                      // [round] {u, i, j, live} of the round's samples
+    unsigned int* cnt_u;            // [n_users] touches of the row in the round (reset to 0 by the round's grad / apply)
+    unsigned int* cnt_v;            // [n_neg]
+    unsigned int* slot_u;           // [n_users] accumulator slot of a shared row (valid while its count is >= 2)
+    unsigned int* slot_v;           // [n_neg]
+    unsigned int* row_of_slot;      // [cap] the row of each slot: user id, or item id | DET_ITEM
+};
+
+struct DetState {
+    DetPlan plan[2];                // by round parity
+    unsigned long long* acc;        // [cap][k + 1] 2^-40 fixed-point sums of the shared rows; column k = the item bias
+    unsigned int* n_shared;         // [rounds] slots taken by each round
+};
+
+// x + d as the global f32 atomic add computes it (round to nearest, subnormal inputs and results flushed to zero)
+__device__ __forceinline__ float det_fadd(float x, float d)
+{
+    float r;
+    asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(d));
+    return r;
+}
+
+// Where a sample's delta for one element of a row goes: straight into the factor x when the sample is the row's only
+// toucher in the round (a == nullptr), else into the row's accumulator slot a.
+struct DetDst {
+    float* x;
+    unsigned long long* a;
 };
 
 // An update that is not finite or beyond the fixed-point range (|d| >= 2^22) cannot be summed: the element it belongs to
 // becomes NaN at once, so a diverging model shows NaN as under the Hogwild kernels instead of saturated sums.
-__device__ __forceinline__ void det_add(unsigned long long* a, float* x, float d)
+__device__ __forceinline__ void det_put(const DetDst& t, int e, float d, float x)
 {
     if (!(fabsf(d) < 4194304.f)) {
-        atomicExch(reinterpret_cast<unsigned int*>(x), 0x7fc00000u);
+        __stcg(t.x + e, __int_as_float(0x7fc00000));
         return;
     }
     const long long q = __double2ll_rn((double)d * DET_SCALE);
-    if (q) atomicAdd(a, (unsigned long long)q);
-}
-// the element's sum is taken (and cleared) by exactly one of the samples that touched it
-__device__ __forceinline__ void det_apply(unsigned long long* a, float* x)
-{
-    const long long q = (long long)atomicExch(a, 0ull);
-    if (q) atomicAdd(x, (float)((double)q * (1.0 / DET_SCALE)));
+    if (!q) return;
+    if (t.a) atomicAdd(t.a + e, (unsigned long long)q);
+    else __stcg(t.x + e, det_fadd(x, (float)((double)q * (1.0 / DET_SCALE))));
 }
 
-// (u, i) and j of epoch-local sample s: the law of the Hogwild kernels
-__device__ __forceinline__ void det_draw(const BprParams& p, int64_t s_local, int32_t& u, int32_t& i, int32_t& j)
+// the slot's sum q of one element added to the factor's value v, the slot left at zero
+__device__ __forceinline__ void det_apply(unsigned long long* a, float* x, long long q, float v)
 {
-    int64_t ii;
-    draw_sample(p, s_local, ii, j);
-    const int2 pr = __ldg(p.pairs + ii);
-    u = pr.x;
-    i = pr.y;
+    if (!q) return;
+    __stcg(a, 0ull);
+    __stcg(x, det_fadd(v, (float)((double)q * (1.0 / DET_SCALE))));
 }
 
-// one warp per sample of [s_begin, s_end): skip test, score, z, the three row updates into the accumulators
-__global__ void __launch_bounds__(256) bpr_det_grad_kernel(const BprParams p, const DetAcc a, int64_t s_begin, int64_t s_end)
+// the plan's touch of a row that took its count from 1 to 2: the row gets a slot
+__device__ __forceinline__ void det_share(unsigned int* slot, unsigned int* row_of_slot, unsigned int* n_shared,
+                                          int32_t row, unsigned tag)
 {
-    const int lane = threadIdx.x & 31;
-    const int64_t s_loc = s_begin + ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
-    unsigned int n_correct = 0, n_skipped = 0;
-    if (s_loc < s_end) {
-        int32_t u, i, j;
-        det_draw(p, s_loc, u, i, j);
-        // has_non_zero(u, j)  (recom_bpr.pyx:241-243) = key (u, j) in the table
-        const uint64_t key = pair_key(u, j);
-        if (group_has<32>(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask, lane)) {
-            n_skipped = 1;
-        } else {
-            const size_t k = (size_t)p.k;
-            const float* pu = p.U + (size_t)u * k;
-            const float* pi = p.V + (size_t)i * k;
-            const float* pj = p.V + (size_t)j * k;
-            float part = 0.f;
-            for (int e = lane; e < p.k; e += 32) part = fmaf(__ldcg(pu + e), __ldcg(pi + e) - __ldcg(pj + e), part);
-            const float bi = __ldcg(p.B + i), bj = __ldcg(p.B + j);
-            const float score = (bi - bj) + group_sum<32>(part);
-            float z = 1.f;
-            bool update = true;
-            if (p.hinge) {
-                if (score > 0.f) { n_correct = 1; update = false; }
-            } else {
-                z = bpr_z(score, p.exact_exp);
-                n_correct = (z < .5f);
-            }
-            if (update) {
-                const float lr = p.lr, reg = p.reg;
-                for (int e = lane; e < p.k; e += 32) {
-                    const float uf = __ldcg(pu + e), vi = __ldcg(pi + e), vj = __ldcg(pj + e);
-                    det_add(a.U + (size_t)u * k + e, p.U + (size_t)u * k + e, lr * (z * (vi - vj) - reg * uf));
-                    det_add(a.V + (size_t)i * k + e, p.V + (size_t)i * k + e, lr * (z * uf - reg * vi));
-                    det_add(a.V + (size_t)j * k + e, p.V + (size_t)j * k + e, lr * (-z * uf - reg * vj));
-                }
-                if (p.use_bias && lane == 0) {
-                    det_add(a.B + i, p.B + i, lr * (z - reg * bi));
-                    det_add(a.B + j, p.B + j, lr * (-z - reg * bj));
-                }
-            }
-        }
-    }
+    const unsigned s = atomicAdd(n_shared, 1u);
+    slot[row] = s;
+    row_of_slot[s] = tag;
+}
+
+// the row's destination in the grad kernel
+__device__ __forceinline__ DetDst det_dst(float* x, const unsigned int* cnt, const unsigned int* slot, int32_t row,
+                                          unsigned long long* acc, int k)
+{
+    DetDst t{x, nullptr};
+    if (__ldcg(cnt + row) >= 2u) t.a = acc + (size_t)__ldcg(slot + row) * (size_t)(k + 1);
+    return t;
+}
+
+// Block epilogue of the deterministic kernels: (correct, skipped) added to the epoch statistics, only when non-zero
+__device__ __forceinline__ void det_flush_stats(unsigned int correct, unsigned int skipped, unsigned long long* stats)
+{
     __shared__ unsigned int sh_stats[2];
     if (threadIdx.x < 2) sh_stats[threadIdx.x] = 0;
     __syncthreads();
-    if (lane == 0 && (n_correct | n_skipped)) {
-        atomicAdd(&sh_stats[0], n_correct);
-        atomicAdd(&sh_stats[1], n_skipped);
+    correct = __reduce_add_sync(0xffffffffu, correct);
+    skipped = __reduce_add_sync(0xffffffffu, skipped);
+    if ((threadIdx.x & 31) == 0 && (correct | skipped)) {
+        atomicAdd(&sh_stats[0], correct);
+        atomicAdd(&sh_stats[1], skipped);
     }
     __syncthreads();
     if (threadIdx.x == 0 && (sh_stats[0] | sh_stats[1])) {
-        atomicAdd(p.stats + 0, (unsigned long long)sh_stats[0]);
-        atomicAdd(p.stats + 1, (unsigned long long)sh_stats[1]);
+        atomicAdd(stats + 0, (unsigned long long)sh_stats[0]);
+        atomicAdd(stats + 1, (unsigned long long)sh_stats[1]);
     }
 }
 
-// one warp per sample of the same round: the summed updates of its rows, each element applied once
-__global__ void __launch_bounds__(256) bpr_det_apply_kernel(const BprParams p, const DetAcc a, int64_t s_begin, int64_t s_end)
+// One warp per record of the round (parity `par`, n records): score, z, and the three row updates.  Lane l owns the
+// elements l, l + 32, ...; the first DET_RC of them stay in registers between the dot and the update.
+constexpr int DET_RC = 4;
+
+__global__ void __launch_bounds__(256, 4) bpr_det_grad_kernel(const BprParams p, const DetState d, int64_t n, int par)
 {
     const int lane = threadIdx.x & 31;
-    const int64_t s_loc = s_begin + ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
-    if (s_loc >= s_end) return;
-    int32_t u, i, j;
-    det_draw(p, s_loc, u, i, j);
-    const size_t k = (size_t)p.k;
-    for (int e = lane; e < p.k; e += 32) {
-        det_apply(a.U + (size_t)u * k + e, p.U + (size_t)u * k + e);
-        det_apply(a.V + (size_t)i * k + e, p.V + (size_t)i * k + e);
-        det_apply(a.V + (size_t)j * k + e, p.V + (size_t)j * k + e);
+    const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
+    const DetPlan pl = par ? d.plan[1] : d.plan[0];
+    unsigned int n_correct = 0;
+    if (w < n) {
+        const int4 r = __ldcg(pl.rec + w);
+        if (r.w) {
+            const int32_t u = r.x, i = r.y, j = r.z;
+            const int k = p.k;
+            float* pu = p.U + (size_t)u * k;
+            float* pi = p.V + (size_t)i * k;
+            float* pj = p.V + (size_t)j * k;
+            float ru[DET_RC], ri[DET_RC], rj[DET_RC];
+#pragma unroll
+            for (int x = 0; x < DET_RC; ++x) {
+                const int e = lane + 32 * x;
+                ru[x] = ri[x] = rj[x] = 0.f;
+                if (e < k) { ru[x] = __ldcg(pu + e); ri[x] = __ldcg(pi + e); rj[x] = __ldcg(pj + e); }
+            }
+            const float bi = __ldcg(p.B + i), bj = __ldcg(p.B + j);
+            const DetDst du = det_dst(pu, pl.cnt_u, pl.slot_u, u, d.acc, k);
+            const DetDst di = det_dst(pi, pl.cnt_v, pl.slot_v, i, d.acc, k);
+            const DetDst dj = det_dst(pj, pl.cnt_v, pl.slot_v, j, d.acc, k);
+            float part = 0.f;
+#pragma unroll
+            for (int x = 0; x < DET_RC; ++x)
+                if (lane + 32 * x < k) part = fmaf(ru[x], ri[x] - rj[x], part);
+            for (int e = lane + 32 * DET_RC; e < k; e += 32) part = fmaf(__ldcg(pu + e), __ldcg(pi + e) - __ldcg(pj + e), part);
+            const float score = (bi - bj) + group_sum<32>(part);
+            float z;
+            if (sample_z(p.hinge, p.exact_exp, score, z, n_correct)) {
+                const float lr = p.lr, reg = p.reg;
+                auto step = [&](int e, float uf, float vi, float vj) {
+                    det_put(du, e, lr * (z * (vi - vj) - reg * uf), uf);
+                    det_put(di, e, lr * (z * uf - reg * vi), vi);
+                    det_put(dj, e, lr * (-z * uf - reg * vj), vj);
+                };
+#pragma unroll
+                for (int x = 0; x < DET_RC; ++x)
+                    if (lane + 32 * x < k) step(lane + 32 * x, ru[x], ri[x], rj[x]);
+                for (int e = lane + 32 * DET_RC; e < k; e += 32) step(e, __ldcg(pu + e), __ldcg(pi + e), __ldcg(pj + e));
+                if (p.use_bias && lane == 0) {
+                    det_put(DetDst{p.B + i, di.a ? di.a + k : nullptr}, 0, lr * (z - reg * bi), bi);
+                    det_put(DetDst{p.B + j, dj.a ? dj.a + k : nullptr}, 0, lr * (-z - reg * bj), bj);
+                }
+            }
+            // a row touched once is reset by its only toucher, after every lane has read its count
+            __syncwarp();
+            if (lane == 0) {
+                if (!du.a) pl.cnt_u[u] = 0u;
+                if (!di.a) pl.cnt_v[i] = 0u;
+                if (!dj.a) pl.cnt_v[j] = 0u;
+            }
+        }
     }
-    if (p.use_bias && lane == 0) {
-        det_apply(a.B + i, p.B + i);
-        det_apply(a.B + j, p.B + j);
+    det_flush_stats(lane == 0 ? n_correct : 0u, 0u, p.stats);      // one count per warp
+}
+
+// Apply of round r (parity par; r < 0: nothing to apply) and plan of the next round (next_n samples from epoch-local
+// next_s0 into parity par ^ 1).  Threads plan one sample each; warps then grid-stride over the slots of round r.
+__global__ void __launch_bounds__(256) bpr_det_apply_kernel(const BprParams p, const DetState d, int64_t r, int par,
+                                                            int64_t next_s0, int64_t next_n)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned int n_skipped = 0;
+    if (t < next_n) {
+        const DetPlan nx = par ? d.plan[0] : d.plan[1];
+        int64_t ii;
+        int32_t j;
+        draw_sample(p, next_s0 + t, ii, j);
+        const int2 pr = __ldg(p.pairs + ii);
+        const uint64_t key = pair_key(pr.x, j);
+        const bool skip = bucket_has(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask);    // recom_bpr.pyx:241-243
+        __stcg(nx.rec + t, make_int4(pr.x, pr.y, j, !skip));
+        if (skip) {
+            n_skipped = 1;
+        } else {
+            // the three counts first (independent round trips), then the slots of the rows that became shared
+            const unsigned cu = atomicAdd(nx.cnt_u + pr.x, 1u);
+            const unsigned ci = atomicAdd(nx.cnt_v + pr.y, 1u);
+            const unsigned cj = atomicAdd(nx.cnt_v + j, 1u);
+            unsigned int* ns = d.n_shared + (r + 1);
+            if (cu == 1u) det_share(nx.slot_u, nx.row_of_slot, ns, pr.x, (unsigned)pr.x);
+            if (ci == 1u) det_share(nx.slot_v, nx.row_of_slot, ns, pr.y, (unsigned)pr.y | DET_ITEM);
+            if (cj == 1u) det_share(nx.slot_v, nx.row_of_slot, ns, j, (unsigned)j | DET_ITEM);
+        }
     }
+    if (r >= 0) {
+        const DetPlan pl = par ? d.plan[1] : d.plan[0];
+        const unsigned n_sh = __ldcg(d.n_shared + r);
+        const int k = p.k;
+        const unsigned n_warps = gridDim.x * (blockDim.x / 32);
+        for (unsigned s = (unsigned)(t / 32); s < n_sh; s += n_warps) {
+            const unsigned tag = __ldcg(pl.row_of_slot + s);
+            const int32_t row = (int32_t)(tag & ~DET_ITEM);
+            const bool item = tag & DET_ITEM;
+            float* x = (item ? p.V : p.U) + (size_t)row * k;
+            unsigned long long* a = d.acc + (size_t)s * (size_t)(k + 1);
+            for (int e0 = 0; e0 < k; e0 += 32 * DET_RC) {       // DET_RC elements per lane in flight at once
+                long long q[DET_RC];
+                float v[DET_RC];
+#pragma unroll
+                for (int c = 0; c < DET_RC; ++c) {
+                    const int e = e0 + lane + 32 * c;
+                    q[c] = 0;
+                    if (e < k) { q[c] = (long long)__ldcg(a + e); v[c] = __ldcg(x + e); }
+                }
+#pragma unroll
+                for (int c = 0; c < DET_RC; ++c) {
+                    const int e = e0 + lane + 32 * c;
+                    if (e < k) det_apply(a + e, x + e, q[c], v[c]);
+                }
+            }
+            if (lane == 0) {
+                if (item && p.use_bias) det_apply(a + k, p.B + row, (long long)__ldcg(a + k), __ldcg(p.B + row));
+                (item ? pl.cnt_v : pl.cnt_u)[row] = 0u;
+            }
+        }
+    }
+    det_flush_stats(0u, n_skipped, p.stats);
 }
 
 static int bpr_epoch_deterministic(const BprParams& p, int64_t n_users, cudaStream_t st)
 {
     const int64_t round = p.max_groups < DET_ROUND ? p.max_groups : DET_ROUND;
-    const size_t nu = (size_t)n_users * p.k, nv = (size_t)p.n_neg * p.k;
-    const size_t bytes = (nu + nv + (size_t)p.n_neg) * sizeof(unsigned long long);
-    void* buf = nullptr;
-    B200_CUDA(cudaMallocAsync(&buf, bytes, st));
-    DetAcc a;
-    a.U = static_cast<unsigned long long*>(buf);
-    a.V = a.U + nu;
-    a.B = a.V + nv;
-    cudaError_t e = cudaMemsetAsync(buf, 0, bytes, st);      // the apply kernel leaves every sum it takes at zero
-    const unsigned grid = (unsigned)((round * 32 + 255) / 256);
-    for (int64_t s0 = 0; s0 < p.n_samples && e == cudaSuccess; s0 += round) {
-        const int64_t s1 = s0 + round < p.n_samples ? s0 + round : p.n_samples;
-        const unsigned g = (unsigned)(((s1 - s0) * 32 + 255) / 256);
-        bpr_det_grad_kernel<<<g < grid ? g : grid, 256, 0, st>>>(p, a, s0, s1);
-        bpr_det_apply_kernel<<<g < grid ? g : grid, 256, 0, st>>>(p, a, s0, s1);
+    const int64_t n_rounds = (p.n_samples + round - 1) / round;
+    const int64_t cap = 3 * round / 2;                 // a shared row takes >= 2 of the round's <= 3 round touches
+    const size_t n_rows = (size_t)n_users + (size_t)p.n_neg;
+    // one stream-ordered buffer: records | accumulators, slot counts, touch counters (zeroed) | slots
+    const size_t rec_b = 2 * (size_t)round * sizeof(int4);
+    const size_t acc_b = (size_t)cap * (size_t)(p.k + 1) * sizeof(unsigned long long);
+    const size_t zero_b = acc_b + (size_t)n_rounds * sizeof(unsigned int) + 2 * n_rows * sizeof(unsigned int);
+    const size_t bytes = rec_b + zero_b + 2 * (n_rows + (size_t)cap) * sizeof(unsigned int);
+    char* buf = nullptr;
+    B200_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), bytes, st));
+    DetState d;
+    d.acc = reinterpret_cast<unsigned long long*>(buf + rec_b);
+    d.n_shared = reinterpret_cast<unsigned int*>(buf + rec_b + acc_b);
+    unsigned int* cnt = d.n_shared + n_rounds;
+    unsigned int* slot = cnt + 2 * n_rows;
+    unsigned int* ros = slot + 2 * n_rows;
+    for (int q = 0; q < 2; ++q) {
+        DetPlan& pl = d.plan[q];
+        pl.rec = reinterpret_cast<int4*>(buf) + q * round;
+        pl.cnt_u = cnt + q * n_rows;
+        pl.cnt_v = pl.cnt_u + n_users;
+        pl.slot_u = slot + q * n_rows;
+        pl.slot_v = pl.slot_u + n_users;
+        pl.row_of_slot = ros + q * cap;
+    }
+    cudaError_t e = cudaMemsetAsync(buf + rec_b, 0, zero_b, st);      // every round leaves counters and slots at zero
+    // apply grid: one thread per sample of the next round's plan, and at least one resident grid of warps (capped by the
+    // slots a round can have) for the shared rows
+    const int64_t apply_min = std::min<int64_t>((int64_t)sm_count() * (2048 / 256), (cap * 32 + 255) / 256);
+    auto blocks = [](int64_t threads) { return (unsigned)((threads + 255) / 256); };
+    if (e == cudaSuccess) {
+        bpr_det_apply_kernel<<<blocks(std::min(round, p.n_samples)), 256, 0, st>>>(p, d, -1, 1, 0,
+                                                                                  std::min(round, p.n_samples));
+        ::b200::count_launch();
+        e = cudaGetLastError();
+    }
+    for (int64_t r = 0; r < n_rounds && e == cudaSuccess; ++r) {
+        const int64_t s0 = r * round;
+        const int64_t n = std::min(round, p.n_samples - s0);
+        const int64_t next_n = r + 1 < n_rounds ? std::min(round, p.n_samples - s0 - round) : 0;
+        const int par = (int)(r & 1);
+        bpr_det_grad_kernel<<<blocks(n * 32), 256, 0, st>>>(p, d, n, par);
+        bpr_det_apply_kernel<<<(unsigned)std::max<int64_t>(blocks(next_n), apply_min), 256, 0, st>>>(p, d, r, par,
+                                                                                                    s0 + round, next_n);
         ::b200::count_launch(2);
         e = cudaGetLastError();
     }
