@@ -8,7 +8,7 @@ Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b
 plug-ins).  The plug-in classes need the `cornac` package importable (they subclass its
 Recommender so that cornac.Experiment accepts them); the engine does not.
 """
-__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "engine", "B200Error"]
+__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "engine", "B200Error"]
 
 from ._lib import B200Error  # noqa: F401
 
@@ -44,6 +44,9 @@ def __getattr__(name):
     if name == "NMF":
         from .recom_nmf import NMF
         return NMF
+    if name == "EASE":
+        from .recom_ease import EASE
+        return EASE
     if name == "BaselineOnly":
         from .recom_bo import BaselineOnly
         return BaselineOnly

@@ -67,6 +67,12 @@ SIGNATURES = {
     "b200_nmf_prepare": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200_nmf_fit": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _int,
                             _vp, _vp, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _f32, _f32, _f32, _int, _vp, _vp]),
+    "b200_ease_gram_workspace_bytes": (_i64, [_i64]),
+    "b200_ease_gram": (_int, [_i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _c.c_double, _vp, _vp, _vp]),
+    "b200_spd_inverse_workspace_bytes": (_i64, [_i64]),
+    "b200_spd_inverse": (_int, [_i64, _vp, _vp, _vp, _int, _vp]),
+    "b200_ease_weights": (_int, [_i64, _vp, _vp, _int, _vp]),
+    "b200_ease_score": (_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),
@@ -99,6 +105,7 @@ BPR_LOSS_HINGE = 16
 BPR_BLOCKED = 32
 BPR_DETERMINISTIC = 64
 PMF_LINEAR, PMF_NON_LINEAR = 0, 1
+SPD_POTRF, SPD_TRTRI, SPD_LAUUM, SPD_ALL = 1, 2, 4, 7
 METRIC_NDCG, METRIC_PRECISION, METRIC_RECALL, METRIC_FMEASURE, METRIC_HIT, METRIC_NCRR = range(6)
 
 _lib = None

@@ -269,3 +269,156 @@ class DeviceScoringMixin:
         in_top[top] = True
         rest = item_indices[~in_top[item_indices]]
         return np.concatenate([top, rest]), item_scores
+
+
+class F64RankingMixin:
+    """`score()` rows, `rank()`, `rank_batch()`, `recommend_batch()` and the `transform()` cache of the models whose score
+    rows are f64 (PMF, EASE), ranked on the device by b200_topk_rows_f64 in the order (score desc, item id asc).  The
+    subclass provides `_scores_dev(user_indices)`: the [n_q, num_items] f64 device score rows of known users."""
+
+    _B200_IGNORED = ("_b200_dev", "_b200_eval_cache")
+    _B200_EVAL_CACHE_BYTES = 1 << 30            # host budget of the transform() cache (f64 score rows of the test users)
+    _B200_EVAL_TOP = 1024                       # length of the cached per-user global ranking
+
+    def _b200_register_f64(self):
+        for a in self._B200_IGNORED:
+            if a not in self.ignored_attrs:
+                self.ignored_attrs.append(a)
+        self._b200_dev = None
+        self._b200_eval_cache = None
+
+    # ---- Recommender.transform: the score rows and ranking heads of every test user --------------------------------
+    def transform(self, test_set):
+        """`Recommender.transform` hook (cornac/models/recommender.py:410-421), called once by BaseMethod.evaluate before
+        the per-user loops: the f64 score rows of all users of `test_set` and, per user, the head of the global ranking
+        (score desc, id asc, b200_topk_rows_f64) are computed in a few kernel calls and kept in host memory, so that
+        score(u), rank() and rate() of those users are host work.  Skipped when the rows do not fit the host budget."""
+        self._b200_eval_cache = None
+        if self._B200_EVAL_CACHE_BYTES <= 0:
+            return
+        try:
+            users = np.unique(np.asarray(test_set.uir_tuple[0], dtype=np.int64))
+        except Exception:
+            return
+        users = users[(users >= 0) & (users < self.num_users)]
+        n = self.num_items
+        if len(users) == 0 or n == 0 or len(users) * n * 8 > self._B200_EVAL_CACHE_BYTES:
+            return
+        m_top = min(n, self._B200_EVAL_TOP)
+        rows = np.empty((len(users), n), dtype=np.float64)
+        top = np.empty((len(users), m_top), dtype=np.int32)
+        batch = max(1, (256 << 20) // (8 * n))
+        for b0 in range(0, len(users), batch):
+            ub = users[b0:b0 + batch]
+            sc = self._scores_dev(ub)
+            ids, _ = engine.topk_rows_f64(sc, m_top)
+            rows[b0:b0 + len(ub)] = sc.cpu().numpy()
+            top[b0:b0 + len(ub)] = ids.cpu().numpy()
+        pos_of = np.full(self.num_users, -1, dtype=np.int64)
+        pos_of[users] = np.arange(len(users))
+        self._b200_eval_cache = dict(pos_of=pos_of, scores=rows, top=top)
+
+    def _cached_row(self, user_idx):
+        c = getattr(self, "_b200_eval_cache", None)
+        if c is None or not (0 <= user_idx < len(c["pos_of"])) or c["pos_of"][user_idx] < 0:
+            return None
+        return c["scores"][c["pos_of"][user_idx]]
+
+    def _b200_row(self, user_idx):
+        """A copy of the f64 score row of a known user, from the transform() cache or the device."""
+        row = self._cached_row(user_idx)
+        return row.copy() if row is not None else self._scores_dev([user_idx])[0].cpu().numpy()
+
+    # reference: recommender.py:476-530, with the total order (score desc, item id asc)
+    def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
+        total = self.total_items
+        item_indices = np.arange(self.num_items) if item_indices is None else np.asarray(item_indices)
+        if not self.knows_user(user_idx):                      # score() raises ScoreException: every item gets default_score
+            item_scores = (np.ones(total) * self.default_score())[item_indices]
+            return item_indices[np.lexsort((item_indices, -item_scores))], item_scores
+        row = self._cached_row(user_idx)
+        c = self._b200_eval_cache if row is not None else None
+        if row is None:
+            row_dev = self._scores_dev([user_idx])
+            row = row_dev[0].cpu().numpy()
+        if len(row) == total:
+            all_scores = row
+        else:                                                  # unknown items get the MIN score (:507-511)
+            all_scores = np.ones(total) * np.min(row)
+            all_scores[: len(row)] = row
+        item_scores = all_scores[item_indices]
+        n_cand = len(item_indices)
+        if k == -1 or k >= n_cand or k > 4096:
+            return item_indices[np.lexsort((item_indices, -item_scores))], item_scores
+        topk = None
+        if c is not None:                                      # the first k candidates of the cached global ranking
+            head = c["top"][c["pos_of"][user_idx]]
+            member = np.zeros(total, dtype=bool)
+            member[item_indices] = True
+            surv = head[member[head]]
+            if len(surv) >= k:
+                topk = surv[:k].astype(item_indices.dtype)
+            else:
+                topk = item_indices[np.lexsort((item_indices, -item_scores))[:k]]
+        else:
+            all_dev = torch.from_numpy(np.ascontiguousarray(all_scores)).cuda()[None, :]
+            ex_ptr = ex_idx = None
+            if not (n_cand == total and np.array_equal(item_indices, np.arange(total))):
+                mask = np.ones(total, dtype=bool)
+                mask[item_indices] = False
+                excl = np.flatnonzero(mask).astype(np.int32)
+                ex_ptr = engine.to_device(np.array([0, len(excl)], dtype=np.int64), torch.int64, pinned=False)
+                ex_idx = engine.to_device(excl if len(excl) else np.zeros(1, np.int32), torch.int32, pinned=False)
+            ids, _ = engine.topk_rows_f64(all_dev, int(k), ex_ptr, ex_idx)
+            topk = ids[0].cpu().numpy().astype(item_indices.dtype)
+        in_top = np.zeros(total, dtype=bool)
+        in_top[topk] = True
+        return np.concatenate([topk, item_indices[~in_top[item_indices]]]), item_scores
+
+    # ---- batched rank ------------------------------------------------------------------------------------------------
+    def rank_batch(self, user_indices, k, exclude=None):
+        """Top-k item ids and scores for many users at once: (ids int32 [n_q, k] (-1 padded), scores f64 [n_q, k]) as numpy
+        arrays in the order (score desc, item id asc).  exclude: optional scipy CSR matrix (rows = user index) whose
+        stored columns are removed from each user's candidates (e.g. train_set.csr_matrix)."""
+        user_indices = np.asarray(user_indices, dtype=np.int64)
+        n_q, n = len(user_indices), self.num_items
+        ids_h = np.empty((n_q, int(k)), dtype=np.int32)
+        sc_h = np.empty((n_q, int(k)), dtype=np.float64)
+        batch = max(1, (256 << 20) // (8 * max(n, 1)))
+        for b0 in range(0, n_q, batch):
+            ub = user_indices[b0:b0 + batch]
+            sc = self._scores_dev(ub)
+            ep = ei = None
+            if exclude is not None:
+                sub = exclude[ub].tocsr()
+                sub.sort_indices()
+                ep = engine.to_device(sub.indptr.astype(np.int64), torch.int64)
+                ei = engine.to_device(sub.indices.astype(np.int32) if sub.nnz else np.zeros(1, np.int32), torch.int32)
+            ids, top = engine.topk_rows_f64(sc, int(k), ep, ei)
+            ids_h[b0:b0 + len(ub)] = ids.cpu().numpy()
+            sc_h[b0:b0 + len(ub)] = top.cpu().numpy()
+        return ids_h, sc_h
+
+    def recommend_batch(self, batch_users, k=-1, remove_seen=False, train_set=None):
+        """The batched form of `Recommender.recommend` (cornac/models/recommender.py:532-580): top-k recommendations of
+        many users, in ORIGINAL ids.  Seen items are removed before the top-k.  Returns a list of lists of item ids."""
+        user_idx = [self.uid_map.get(uid, -1) for uid in batch_users]
+        if any(i == -1 for i in user_idx):
+            raise ValueError(f"{batch_users} is unknown to the model.")
+        if k < -1 or k > self.total_items:
+            raise ValueError(f"k={k} is invalid, there are {self.total_users} users in total.")
+        if remove_seen and train_set is None:
+            raise ValueError("train_set must be provided to remove seen items.")
+        if k == -1 or k > 4096 or any(not self.knows_user(u) for u in user_idx):
+            return [self.recommend(uid, k=k, remove_seen=remove_seen, train_set=train_set) for uid in batch_users]
+        exclude = None
+        if remove_seen:
+            exclude = train_set.csr_matrix
+            n_rows = max(user_idx) + 1
+            if exclude.shape[0] < n_rows:                     # users without a training row have nothing to remove
+                import scipy.sparse as sp
+                exclude = sp.vstack([exclude, sp.csr_matrix((n_rows - exclude.shape[0], exclude.shape[1]),
+                                                            dtype=exclude.dtype)]).tocsr()
+        ids, _ = self.rank_batch(np.asarray(user_idx, dtype=np.int64), int(k), exclude=exclude)
+        item_ids = self.item_ids
+        return [[item_ids[i] for i in row if i >= 0] for row in ids]

@@ -31,21 +31,26 @@ __device__ __forceinline__ double amplify_map(double s, double alpha)
     return s > 0.0 ? pow(s, alpha) : -pow(-s, alpha);
 }
 
-// one CTA per row r (persistent, rows in `order`); acc = S, D1, D2 for x in [r, n), in shared memory or the workspace
+// one CTA per row r (persistent, rows in `order`); acc = S, D1, D2 for x in [r, n), in shared memory or the workspace.
+// RAW (EASE's Gram matrix, K10): only S is accumulated, with no normalisation; `param` is then lambda, added to S[r,r].
+template <bool RAW>
 __global__ void __launch_bounds__(SIM_THREADS) knn_sim_kernel(
     int n, const int32_t* __restrict__ rp, const int32_t* __restrict__ ri, const double* __restrict__ rd,
     const int32_t* __restrict__ cp, const int32_t* __restrict__ ci, const double* __restrict__ cd,
-    const int32_t* __restrict__ order, double alpha, double* ws, double* __restrict__ out)
+    const int32_t* __restrict__ order, double param, double* ws, double* __restrict__ out)
 {
     extern __shared__ double smem[];
-    double* S = ws ? ws + (size_t)blockIdx.x * 3 * n : smem;
+    double* S = ws ? ws + (size_t)blockIdx.x * (RAW ? 1 : 3) * n : smem;
     double* D1 = S + n;
     double* D2 = D1 + n;
     const int tid = threadIdx.x;
     for (int t = blockIdx.x; t < n; t += gridDim.x) {
         const int r = __ldg(order + t);
         const int m = n - r;
-        for (int x = tid; x < m; x += SIM_THREADS) S[x] = D1[x] = D2[x] = 0.0;
+        for (int x = tid; x < m; x += SIM_THREADS) {
+            S[x] = 0.0;
+            if (!RAW) D1[x] = D2[x] = 0.0;
+        }
         __syncthreads();
         const int pe = __ldg(rp + r + 1);
         for (int p = __ldg(rp + r); p < pe; ++p) {
@@ -62,7 +67,7 @@ __global__ void __launch_bounds__(SIM_THREADS) knn_sim_kernel(
                 const int x = __ldg(ci + j) - r;
                 const double v = __ldg(cd + j);
                 S[x] = __dadd_rn(S[x], __dmul_rn(v, w));
-                if (w != 0.0 && v != 0.0) {
+                if (!RAW && w != 0.0 && v != 0.0) {
                     D1[x] = __dadd_rn(D1[x], ww);
                     D2[x] = __dadd_rn(D2[x], __dmul_rn(v, v));
                 }
@@ -72,9 +77,11 @@ __global__ void __launch_bounds__(SIM_THREADS) knn_sim_kernel(
         double* row = out + (size_t)r * n + r;
         for (int x = tid; x < m; x += SIM_THREADS) {
             double s = S[x];
-            if (s != 0.0) {
+            if (RAW) {
+                if (x == 0) s = __dadd_rn(s, param);
+            } else if (s != 0.0) {
                 s = __ddiv_rn(s, __dsqrt_rn(__dmul_rn(D1[x], D2[x])));
-                if (alpha != 1.0) s = amplify_map(s, alpha);
+                if (param != 1.0) s = amplify_map(s, param);
             }
             row[x] = s;
         }
@@ -279,7 +286,8 @@ __global__ void knn_score_users_kernel(const int64_t* __restrict__ users, int64_
 }
 
 // ---- launch plans (shared by the workspace queries and the launches) ----
-static bool sim_in_smem(int64_t n) { return (size_t)n * 3 * sizeof(double) <= SMEM_LIMIT; }
+static int sim_accs(bool raw) { return raw ? 1 : 3; }
+static bool sim_in_smem(int64_t n, bool raw) { return (size_t)n * sim_accs(raw) * sizeof(double) <= SMEM_LIMIT; }
 
 struct ScorePlan {
     int threads;       // block size
@@ -314,43 +322,66 @@ static ScorePlan score_plan(int64_t n_q, int64_t n_stage, int k)
 
 using namespace b200;
 
-extern "C" int64_t b200_knn_similarity_workspace_bytes(int64_t n)
+static int64_t sim_workspace_bytes(int64_t n, bool raw)
 {
-    if (n <= 0 || knn::sim_in_smem(n)) return 0;
+    if (n <= 0 || knn::sim_in_smem(n, raw)) return 0;
     const int64_t ctas = n < knn::SIM_WS_CTAS ? n : knn::SIM_WS_CTAS;
-    return ctas * 3 * n * (int64_t)sizeof(double);
+    return ctas * knn::sim_accs(raw) * n * (int64_t)sizeof(double);
 }
 
-extern "C" int b200_knn_similarity(int64_t n, const int32_t* row_indptr, const int32_t* row_indices, const double* row_data,
-                                   int64_t n_cols, const int32_t* col_indptr, const int32_t* col_indices, const double* col_data,
-                                   const int32_t* order, double amplify, void* workspace, double* out, void* stream)
+// the ordered row-pair sums of knn_sim_kernel<RAW> for x >= r, then the mirror of the lower triangle
+template <bool RAW>
+static int sim_launch(int64_t n, const int32_t* row_indptr, const int32_t* row_indices, const double* row_data, int64_t n_cols,
+                      const int32_t* col_indptr, const int32_t* col_indices, const double* col_data, const int32_t* order,
+                      double param, void* workspace, double* out, void* stream, const char* what)
 {
-    B200_REQUIRE(n >= 1 && n < (1LL << 31) && n_cols >= 1 && n_cols < (1LL << 31), "b200_knn_similarity: bad sizes n=%lld n_cols=%lld",
+    B200_REQUIRE(n >= 1 && n < (1LL << 31) && n_cols >= 1 && n_cols < (1LL << 31), "%s: bad sizes n=%lld n_cols=%lld", what,
                  (long long)n, (long long)n_cols);
     B200_REQUIRE(row_indptr && row_indices && row_data && col_indptr && col_indices && col_data && order && out,
-                 "b200_knn_similarity: null pointer argument");
-    const bool smem = knn::sim_in_smem(n);
-    B200_REQUIRE(smem || workspace, "b200_knn_similarity: n=%lld needs a workspace of %lld bytes", (long long)n,
-                 (long long)b200_knn_similarity_workspace_bytes(n));
+                 "%s: null pointer argument", what);
+    const bool smem = knn::sim_in_smem(n, RAW);
+    B200_REQUIRE(smem || workspace, "%s: n=%lld needs a workspace of %lld bytes", what, (long long)n,
+                 (long long)sim_workspace_bytes(n, RAW));
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t sm_bytes = smem ? (size_t)n * 3 * sizeof(double) : 0;
+    const size_t sm_bytes = smem ? (size_t)n * knn::sim_accs(RAW) * sizeof(double) : 0;
     int grid;
     if (smem) {
-        B200_CUDA(cudaFuncSetAttribute(knn::knn_sim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_bytes));
+        B200_CUDA(cudaFuncSetAttribute(knn::knn_sim_kernel<RAW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_bytes));
         int per_sm = 0;
-        B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, knn::knn_sim_kernel, knn::SIM_THREADS, sm_bytes));
+        B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, knn::knn_sim_kernel<RAW>, knn::SIM_THREADS, sm_bytes));
         const int64_t cap = (int64_t)sm_count() * (per_sm > 0 ? per_sm : 1);
         grid = (int)(n < cap ? n : cap);
     } else {
         grid = (int)(n < knn::SIM_WS_CTAS ? n : knn::SIM_WS_CTAS);
     }
-    knn::knn_sim_kernel<<<grid, knn::SIM_THREADS, sm_bytes, st>>>((int)n, row_indptr, row_indices, row_data, col_indptr,
-                                                                  col_indices, col_data, order, amplify,
-                                                                  smem ? nullptr : (double*)workspace, out); ::b200::count_launch();
+    knn::knn_sim_kernel<RAW><<<grid, knn::SIM_THREADS, sm_bytes, st>>>((int)n, row_indptr, row_indices, row_data, col_indptr,
+                                                                       col_indices, col_data, order, param,
+                                                                       smem ? nullptr : (double*)workspace, out);
+    ::b200::count_launch();
     const unsigned tiles = (unsigned)((n + 31) / 32);
     knn::knn_mirror_kernel<<<dim3(tiles, tiles), dim3(32, 8), 0, st>>>((int)n, out); ::b200::count_launch();
     B200_CUDA(cudaGetLastError());
     return B200_OK;
+}
+
+extern "C" int64_t b200_knn_similarity_workspace_bytes(int64_t n) { return sim_workspace_bytes(n, false); }
+
+extern "C" int b200_knn_similarity(int64_t n, const int32_t* row_indptr, const int32_t* row_indices, const double* row_data,
+                                   int64_t n_cols, const int32_t* col_indptr, const int32_t* col_indices, const double* col_data,
+                                   const int32_t* order, double amplify, void* workspace, double* out, void* stream)
+{
+    return sim_launch<false>(n, row_indptr, row_indices, row_data, n_cols, col_indptr, col_indices, col_data, order, amplify,
+                             workspace, out, stream, "b200_knn_similarity");
+}
+
+extern "C" int64_t b200_ease_gram_workspace_bytes(int64_t n) { return sim_workspace_bytes(n, true); }
+
+extern "C" int b200_ease_gram(int64_t n, const int32_t* row_indptr, const int32_t* row_indices, const double* row_data,
+                              int64_t n_cols, const int32_t* col_indptr, const int32_t* col_indices, const double* col_data,
+                              const int32_t* order, double lamb, void* workspace, double* out, void* stream)
+{
+    return sim_launch<true>(n, row_indptr, row_indices, row_data, n_cols, col_indptr, col_indices, col_data, order, lamb,
+                            workspace, out, stream, "b200_ease_gram");
 }
 
 extern "C" int b200_knn_row_nnz(int64_t n, const double* sim, int32_t* counts, void* stream)

@@ -11,6 +11,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     pmf_schedule / pmf_fit         <-> pmf_linear / pmf_non_linear (cornac/models/pmf/cython/pmf.pyx:55-173)
     score_batch_f64 / topk_rows_f64 <-> PMF.score / Recommender.rank (cornac/models/pmf/recom_pmf.py:191-222)
     nmf_prepare / nmf_fit          <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
+    ease_fit / ease_score          <-> EASE.fit / EASE.score (cornac/models/ease/recom_ease.py:57-126)
 """
 import numpy as np
 import scipy.sparse as _sp
@@ -465,6 +466,16 @@ def _upload_csr(m, what):
     return to_device(ip, torch.int32), to_device(ix, torch.int32), to_device(dt, torch.float64)
 
 
+def _heaviest_rows_first(rows, cols):
+    """The rows of `rows` in decreasing work (sum of the lengths of the rows of `cols` a row touches), so that the longest
+    rows of an ordered row-pair sum start first."""
+    ip, ix, _ = _csr_arrays(rows, "weight matrix")
+    work = np.zeros(len(ip) - 1, dtype=np.int64)
+    if len(ix):
+        np.add.at(work, np.repeat(np.arange(len(ip) - 1), np.diff(ip)), np.diff(cols.indptr)[ix])
+    return np.argsort(-work, kind="stable").astype(np.int32)
+
+
 def knn_similarity(weight, amplify=1.0):
     """compute_similarity + the amplify map (cornac/models/knn/similarity.pyx:51-105, recom_knn.py:48-55) of the rows of
     the scipy CSR weight matrix.  Returns (S, sim_mat): the dense symmetric f64 [n, n] device similarity and the same
@@ -480,12 +491,7 @@ def knn_similarity(weight, amplify=1.0):
                         % (n, n, need, ws_bytes, free))
     cols = weight.T.tocsr()
     cols.sort_indices()
-    ip, ix, _ = _csr_arrays(weight, "weight matrix")
-    # rows in decreasing work (sum of the lengths of the columns a row touches), so the longest rows start first
-    work = np.zeros(n, dtype=np.int64)
-    if len(ix):
-        np.add.at(work, np.repeat(np.arange(n), np.diff(ip)), np.diff(cols.indptr)[ix])
-    order = np.argsort(-work, kind="stable").astype(np.int32)
+    order = _heaviest_rows_first(weight, cols)
     r_p, r_i, r_d = _upload_csr(weight, "weight matrix")
     c_p, c_i, c_d = _upload_csr(cols, "weight matrix")
     ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device="cuda")
@@ -508,6 +514,144 @@ def knn_similarity(weight, amplify=1.0):
     check(L.b200_knn_compact(n, ptr(S), ptr(d_ptr), ptr(d_idx), ptr(d_val), st), "b200_knn_compact")
     sim = _sp.csr_matrix((d_val[:nnz].cpu().numpy(), d_idx[:nnz].cpu().numpy(), indptr.astype(np.int32)), shape=(n, n))
     return S, sim
+
+
+def _csr_bytes(n_rows, nnz):
+    """Device bytes of an int32 / int32 / f64 CSR copy (_upload_csr)."""
+    return 4 * (n_rows + 1) + 12 * max(nnz, 1)
+
+
+def ease_device_bytes(n_users, n_items, nnz):
+    """Device bytes of ease_fit plus the rating copy the scores read: the n x n matrix, the Gram inputs (X^T and X as CSR,
+    the row order) and workspace, the inverse workspace, the saved diagonal, and EaseRatings."""
+    L = _lib.load()
+    n = int(n_items)
+    return (n * n * 8 + _csr_bytes(n, nnz) + _csr_bytes(n_users, nnz) + 4 * n + int(L.b200_ease_gram_workspace_bytes(n))
+            + int(L.b200_spd_inverse_workspace_bytes(n)) + 8 * n + _csr_bytes(n_users, nnz))
+
+
+class EaseGramInput:
+    """The device inputs of b200_ease_gram for a scipy CSR rating matrix X (users x items): X^T as CSR with each item's
+    users ascending (the order of scipy's sums), X as CSR with each user's items ascending, and the item rows in
+    decreasing work.  Built once; ease_gram then only launches."""
+
+    def __init__(self, X):
+        require_cuda()
+        X = X.tocsr().copy()
+        X.sort_indices()
+        self.n_users, self.n = (int(x) for x in X.shape)
+        XT = X.T.tocsr()
+        XT.sort_indices()
+        self.rows = _upload_csr(XT, "rating matrix")
+        self.cols = _upload_csr(X, "rating matrix")
+        self.order = to_device(_heaviest_rows_first(XT, X), torch.int32)
+
+
+def ease_gram(inp, lamb, out, workspace=None):
+    """X.T.dot(X).toarray() + lamb on the diagonal into the f64 device tensor out [n_items, n_items], bit for bit (the
+    raw mode of the KNN similarity kernel over the rows of X^T).  inp: EaseGramInput of X."""
+    L = require_cuda()
+    n = inp.n
+    _dev(out, torch.float64, "out")
+    if tuple(out.shape) != (n, n):
+        raise B200Error("out must have shape (%d, %d)" % (n, n))
+    ws_bytes = int(L.b200_ease_gram_workspace_bytes(n))
+    if workspace is None and ws_bytes:
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
+    (r_p, r_i, r_d), (c_p, c_i, c_d) = inp.rows, inp.cols
+    check(L.b200_ease_gram(n, ptr(r_p), ptr(r_i), ptr(r_d), max(inp.n_users, 1), ptr(c_p), ptr(c_i), ptr(c_d),
+                           ptr(inp.order), float(lamb), ptr(workspace) if ws_bytes else None, ptr(out), current_stream()),
+          "b200_ease_gram")
+    return out
+
+
+def spd_inverse(A, phases=_lib.SPD_ALL, workspace=None, info=None):
+    """Replace the symmetric positive definite f64 device matrix A [n, n] (lower triangle read) by its inverse, in place, on
+    the FP64 tensor cores (b200_spd_inverse).  `phases` runs a subset of potrf / trtri / lauum (in order, with the same
+    workspace and info).  Raises numpy.linalg.LinAlgError naming the first failing column when A is not positive definite
+    (checked after the factorisation; the call then synchronises with the device)."""
+    L = require_cuda()
+    _dev(A, torch.float64, "A")
+    n = int(A.shape[0])
+    if A.dim() != 2 or int(A.shape[1]) != n:
+        raise B200Error("A must be square, got %s" % (tuple(A.shape),))
+    if workspace is None:
+        workspace = torch.empty(int(L.b200_spd_inverse_workspace_bytes(n)), dtype=torch.uint8, device="cuda")
+    if info is None:
+        info = torch.zeros(1, dtype=torch.int32, device="cuda")
+    check(L.b200_spd_inverse(n, ptr(A), ptr(workspace), ptr(info), int(phases), current_stream()), "b200_spd_inverse")
+    if phases & _lib.SPD_POTRF:
+        bad = int(info.item())
+        if bad:
+            raise np.linalg.LinAlgError("the %d x %d Gram matrix is not positive definite: pivot of column %d is not a "
+                                        "positive finite number (info = %d)" % (n, n, bad - 1, bad))
+    return A
+
+
+def ease_weights(P, posB, diag=None):
+    """B = P / -diag(P), B[j, j] = 0, negatives to 0 under posB, in place on the f64 device matrix P (b200_ease_weights)."""
+    L = require_cuda()
+    _dev(P, torch.float64, "P")
+    n = int(P.shape[0])
+    if diag is None:
+        diag = torch.empty(n, dtype=torch.float64, device="cuda")
+    check(L.b200_ease_weights(n, ptr(P), ptr(diag), int(bool(posB)), current_stream()), "b200_ease_weights")
+    return P
+
+
+def ease_fit(X, lamb, posB):
+    """EASE.fit (recom_ease.py:72-95) on the device: G = X^T X + lamb I, P = G^-1, B = P / -diag(P).  Returns B, the f64
+    device [n_items, n_items] weight matrix.  Refuses before allocating when it does not fit the free device memory;
+    raises numpy.linalg.LinAlgError when G is not positive definite (only possible for lamb <= 0)."""
+    require_cuda()
+    n_users, n = (int(x) for x in X.shape)
+    need = ease_device_bytes(n_users, n, X.nnz)
+    free, _ = torch.cuda.mem_get_info()
+    free += torch.cuda.memory_reserved() - torch.cuda.memory_allocated()    # blocks torch's allocator holds but does not use
+    if need > free:
+        raise B200Error("the dense %d x %d f64 EASE matrix needs %d bytes with its inputs and workspaces (%d bytes in all); the "
+                        "device has %d bytes free" % (n, n, n * n * 8, need, free))
+    inp = EaseGramInput(X)
+    B = torch.empty((n, n), dtype=torch.float64, device="cuda")
+    ease_gram(inp, lamb, B)
+    del inp
+    spd_inverse(B)
+    return ease_weights(B, posB)
+
+
+class EaseRatings:
+    """Device copy of the CSR rating matrix X that EASE's score rows read, in stored order."""
+
+    def __init__(self, X):
+        require_cuda()
+        X = X.tocsr()
+        self.n_rows, self.n_cols = (int(x) for x in X.shape)
+        self.indptr, self.indices, self.data = _upload_csr(X, "rating matrix")
+
+
+def ease_score(B, users, ratings, out=None):
+    """out[q, :] = X[users[q], :] . B in scipy's order (b200_ease_score): f64 [n_q, n_items] device score rows.
+    ratings: EaseRatings of X; B: f64 device [n_items, n_items]; users: indices of rows of X (host or int64 device)."""
+    L = require_cuda()
+    _dev(B, torch.float64, "B")
+    n = int(B.shape[0])
+    if B.dim() != 2 or int(B.shape[1]) != n or n != ratings.n_cols:
+        raise B200Error("B must be square with one row per item of the ratings (%d), got %s" % (ratings.n_cols, tuple(B.shape)))
+    if isinstance(users, torch.Tensor):
+        _dev(users, torch.int64, "users")
+        lo, hi = (int(users.min()), int(users.max())) if users.numel() else (0, 0)
+    else:
+        host = np.asarray(users, dtype=np.int64)
+        lo, hi = (int(host.min()), int(host.max())) if host.size else (0, 0)
+        users = to_device(host, torch.int64)
+    if lo < 0 or hi >= ratings.n_rows:
+        raise B200Error("user index out of range [0, %d): %d" % (ratings.n_rows, lo if lo < 0 else hi))
+    n_q = int(users.numel())
+    if out is None:
+        out = torch.empty((n_q, n), dtype=torch.float64, device="cuda")
+    check(L.b200_ease_score(ptr(users), n_q, n, ptr(ratings.indptr), ptr(ratings.indices), ptr(ratings.data), ptr(B),
+                            ptr(_dev(out, torch.float64, "out")), current_stream()), "b200_ease_score")
+    return out
 
 
 def knn_dense(sim):

@@ -336,6 +336,45 @@ B200_API int b200_nmf_fit(const int32_t* indptr, const int32_t* indices, const f
                           int use_bias, double* loss, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * EASE (cornac/models/ease/recom_ease.py:57-126): G = X^T X + lamb I, P = G^-1, B = P / -diag(P) with B[j,j] = 0 (and
+ * negatives to 0 under posB), score(u) = X[u, :] . B.
+ *
+ * b200_ease_gram: out = the dense f64 [n, n] X^T X with lamb added to the diagonal, bit-identical to scipy's
+ *   X.T.dot(X).toarray() + lamb: every entry is the sum over users in ascending order of X[u,a] * X[u,b], each product
+ *   and sum rounded.  Arguments as b200_knn_similarity with row_* = X^T (items x users, users ascending in each row) and
+ *   col_* = X (users x items, items ascending); workspace of b200_ease_gram_workspace_bytes(n) bytes (0 = none needed).
+ *
+ * b200_spd_inverse: A (device f64 [n, n], row-major, lower triangle read) is replaced by its inverse, exactly symmetric,
+ *   through a blocked Cholesky factorisation on the FP64 tensor cores.  The result repeats bit for bit from run to run.
+ *   phases: B200_SPD_ALL, or the bits of the phases to run (in this order; each needs the ones before it):
+ *     B200_SPD_POTRF  A = L L^T, L in the lower triangle
+ *     B200_SPD_TRTRI  Z = L^-T in the upper triangle (the diagonal blocks' lower parts keep stale values)
+ *     B200_SPD_LAUUM  A = Z Z^T = A^-1, both triangles
+ *   info       device int: 0, or (set by B200_SPD_POTRF) the first column j + 1 whose pivot is not a positive finite number
+ *              -- A is then not positive definite and its contents are undefined
+ *   workspace  device scratch of b200_spd_inverse_workspace_bytes(n) bytes, kept between the phases of one inverse
+ *
+ * b200_ease_weights: P (device f64 [n, n]) is replaced by B, element by element as numpy's expression (the diagonal of P
+ *   is saved to diag_workspace, device f64 [n], first).
+ *
+ * b200_ease_score: out[q, :] = X[users[q], :] . B (device f64 [n_q, n_items]), bit-identical to scipy's sparse row times
+ *   dense matrix: acc = +0.0, then acc = acc + x * B[i, :] for the stored (i, x) of the row in stored order, no FMA.
+ *   indptr / indices / data: the CSR of X (int32, int32, f64); B device f64 [n_items, n_items].                          */
+#define B200_SPD_POTRF 1
+#define B200_SPD_TRTRI 2
+#define B200_SPD_LAUUM 4
+#define B200_SPD_ALL 7
+B200_API int64_t b200_ease_gram_workspace_bytes(int64_t n);
+B200_API int b200_ease_gram(int64_t n, const int32_t* row_indptr, const int32_t* row_indices, const double* row_data,
+                            int64_t n_cols, const int32_t* col_indptr, const int32_t* col_indices, const double* col_data,
+                            const int32_t* order, double lamb, void* workspace, double* out, void* stream);
+B200_API int64_t b200_spd_inverse_workspace_bytes(int64_t n);
+B200_API int b200_spd_inverse(int64_t n, double* A, void* workspace, int* info, int phases, void* stream);
+B200_API int b200_ease_weights(int64_t n, double* P, double* diag_workspace, int posB, void* stream);
+B200_API int b200_ease_score(const int64_t* users, int64_t n_q, int64_t n_items, const int32_t* indptr,
+                             const int32_t* indices, const double* data, const double* B, double* out, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
