@@ -822,17 +822,19 @@ static int launch_hogwild(const BprParams& p, cudaStream_t st)
 // that element -- so the order in which the samples run does not matter and a run repeats bit for bit.  A round is about
 // as many samples as the Hogwild kernels keep in flight, so the updates of a popular row are summed against a similar
 // staleness.  Per round r the work is split in three phases, ordered by kernel boundaries on one stream only:
-//   plan   (inside bpr_det_apply_kernel of round r - 1; a prologue launch of the same kernel plans round 0): one thread per
-//          sample draws it, runs the skip test, writes its record {u, i, j, live} and counts the touches of its three rows;
-//          the touch that makes a row SHARED (count 1 -> 2) gives it a slot of a compact accumulator (which row gets which
-//          slot depends on timing, but the sums are exact integers, so it does not change the result);
+//   plan   (in the first CTAs of bpr_det_grad_kernel of round r - 1; a prologue launch of bpr_det_apply_kernel plans
+//          round 0): one thread per sample draws it, runs the skip test, writes its record {u, i, j, live} and counts the
+//          touches of its three rows; the touch that makes a row SHARED (count 1 -> 2) gives it a slot of a compact
+//          accumulator (which row gets which slot depends on timing, but the sums are exact integers, so it does not
+//          change the result);
 //   grad   (bpr_det_grad_kernel): one warp per record computes score, z and the deltas.  A row the sample is the only
 //          toucher of is read by no other sample of the round, so the warp adds its deltas to it at once; the deltas of a
 //          shared row go into the row's slot with integer atomics;
 //   apply  (bpr_det_apply_kernel): one warp per slot adds the slot's sums to its row and clears the slot.
 // A live sample never touches one item row twice (j == i means (u, j) is an interaction: the sample is skipped), so a
 // row touched once receives exactly one term.  The plan state is double-buffered by round parity: the plan of round
-// r + 1 reads only the inputs and writes only the other parity, so it shares nothing with the apply of round r.
+// r + 1 reads only the inputs and writes only the other parity, whose last users (grad and apply of round r - 1) have
+// completed, so it shares nothing with the grad and apply of round r.
 constexpr int64_t DET_ROUND = 16384;
 constexpr double DET_SCALE = 1099511627776.0;       // 2^40
 constexpr unsigned DET_ITEM = 0x80000000u;          // row_of_slot tag of an item row (user rows carry their id alone)
@@ -889,13 +891,60 @@ __device__ __forceinline__ void det_apply(unsigned long long* a, float* x, long 
     __stcg(x, det_fadd(v, (float)((double)q * (1.0 / DET_SCALE))));
 }
 
-// the plan's touch of a row that took its count from 1 to 2: the row gets a slot
-__device__ __forceinline__ void det_share(unsigned int* slot, unsigned int* row_of_slot, unsigned int* n_shared,
-                                          int32_t row, unsigned tag)
+// Programmatic dependent launch: the per-round launches of an epoch may start while the launch before them still runs.
+// Every CTA calls this before its first access to state an earlier launch writes: it waits until the launch before has
+// completed and its writes are visible, and only then lets the next launch start.  So when launch N + 1 starts, every
+// CTA of launch N has passed its wait, and launch N - 1 has completed.  (Without a programmatic dependency the wait
+// returns at once.)
+__device__ __forceinline__ void det_pdl_sync()
 {
-    const unsigned s = atomicAdd(n_shared, 1u);
-    slot[row] = s;
-    row_of_slot[s] = tag;
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
+
+// Plan of sample s0 + t (t < n) into nx, its shared rows taking slots from *n_shared; returns 1 when the sample is
+// skipped.  Every lane of the warp calls it: the draw and the two gathers read only inputs and run before det_pdl_sync,
+// so they overlap the launch before; the touch counters, slots and records of nx come after it.
+__device__ __forceinline__ unsigned det_plan(const BprParams& p, const DetPlan& nx, unsigned int* n_shared, int64_t t,
+                                             int64_t s0, int64_t n)
+{
+    int2 pr = make_int2(0, 0);
+    int32_t j = 0;
+    bool skip = false;
+    if (t < n) {
+        int64_t ii;
+        draw_sample(p, s0 + t, ii, j);
+        pr = __ldg(p.pairs + ii);
+        const uint64_t key = pair_key(pr.x, j);
+        skip = bucket_has(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask);      // recom_bpr.pyx:241-243
+    }
+    det_pdl_sync();
+    unsigned cu = 0, ci = 0, cj = 0;
+    if (t < n) {
+        __stcg(nx.rec + t, make_int4(pr.x, pr.y, j, !skip));
+        if (!skip) {
+            // the three counts (independent round trips); the touch that takes a count from 1 to 2 makes the row shared
+            cu = atomicAdd(nx.cnt_u + pr.x, 1u);
+            ci = atomicAdd(nx.cnt_v + pr.y, 1u);
+            cj = atomicAdd(nx.cnt_v + j, 1u);
+        }
+    }
+    // the warp takes the slots of all its shared rows (0-3 per lane) with one atomic: lane l's first slot is the base plus
+    // the rows of lanes < l, counted from the two bits of each lane's number
+    const bool su = cu == 1u, si = ci == 1u, sj = cj == 1u;
+    const unsigned m = (unsigned)su + (unsigned)si + (unsigned)sj;
+    const unsigned b0 = __ballot_sync(0xffffffffu, m & 1u), b1 = __ballot_sync(0xffffffffu, m & 2u);
+    if (b0 | b1) {
+        const int lane = threadIdx.x & 31;
+        unsigned base = 0;
+        if (lane == 0) base = atomicAdd(n_shared, (unsigned)__popc(b0) + 2u * (unsigned)__popc(b1));
+        const unsigned below = (1u << lane) - 1u;
+        unsigned s = __shfl_sync(0xffffffffu, base, 0) + (unsigned)__popc(b0 & below) + 2u * (unsigned)__popc(b1 & below);
+        if (su) { nx.slot_u[pr.x] = s; nx.row_of_slot[s++] = (unsigned)pr.x; }
+        if (si) { nx.slot_v[pr.y] = s; nx.row_of_slot[s++] = (unsigned)pr.y | DET_ITEM; }
+        if (sj) { nx.slot_v[j] = s; nx.row_of_slot[s] = (unsigned)j | DET_ITEM; }
+    }
+    return skip ? 1u : 0u;
 }
 
 // the row's destination in the grad kernel
@@ -926,20 +975,33 @@ __device__ __forceinline__ void det_flush_stats(unsigned int correct, unsigned i
     }
 }
 
-// One warp per record of the round (parity `par`, n records): score, z, and the three row updates.  Lane l owns the
-// elements l, l + 32, ...; the first DET_RC of them stay in registers between the dot and the update.
+// Grad of round r (parity par, n records) and plan of round r + 1 (next_n samples from epoch-local next_s0 into parity
+// par ^ 1).  The first ceil(next_n / 256) CTAs plan, one sample per thread.  CTAs are expected (not guaranteed) to be
+// dispatched in blockIdx order, so the plan's chains of dependent gathers and atomics overlap the grad CTAs; the result
+// does not depend on it.  The other CTAs run one warp per record: score, z, and the three row updates.  Lane l owns the elements l, l + 32, ...; the first DET_RC of them stay in registers between the dot and the
+// update.
 constexpr int DET_RC = 4;
 
-__global__ void __launch_bounds__(256, 4) bpr_det_grad_kernel(const BprParams p, const DetState d, int64_t n, int par)
+__global__ void __launch_bounds__(256, 4) bpr_det_grad_kernel(const BprParams p, const DetState d, int64_t r, int par,
+                                                              int64_t n, int64_t next_s0, int64_t next_n)
 {
     const int lane = threadIdx.x & 31;
-    const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
+    const unsigned plan_ctas = (unsigned)((next_n + 255) / 256);
+    if (blockIdx.x < plan_ctas) {
+        const DetPlan nx = par ? d.plan[0] : d.plan[1];
+        const unsigned skipped = det_plan(p, nx, d.n_shared + (r + 1), (int64_t)blockIdx.x * blockDim.x + threadIdx.x,
+                                          next_s0, next_n);
+        det_flush_stats(0u, skipped, p.stats);
+        return;
+    }
+    det_pdl_sync();
+    const int64_t w = ((int64_t)(blockIdx.x - plan_ctas) * blockDim.x + threadIdx.x) / 32;
     const DetPlan pl = par ? d.plan[1] : d.plan[0];
     unsigned int n_correct = 0;
     if (w < n) {
-        const int4 r = __ldcg(pl.rec + w);
-        if (r.w) {
-            const int32_t u = r.x, i = r.y, j = r.z;
+        const int4 rec = __ldcg(pl.rec + w);
+        if (rec.w) {
+            const int32_t u = rec.x, i = rec.y, j = rec.z;
             const int k = p.k;
             float* pu = p.U + (size_t)u * k;
             float* pi = p.V + (size_t)i * k;
@@ -990,69 +1052,48 @@ __global__ void __launch_bounds__(256, 4) bpr_det_grad_kernel(const BprParams p,
     det_flush_stats(lane == 0 ? n_correct : 0u, 0u, p.stats);      // one count per warp
 }
 
-// Apply of round r (parity par; r < 0: nothing to apply) and plan of the next round (next_n samples from epoch-local
-// next_s0 into parity par ^ 1).  Threads plan one sample each; warps then grid-stride over the slots of round r.
+// Apply of round r (parity par): warps grid-stride over the round's slots.  The epoch's prologue launch (r < 0) has
+// nothing to apply and plans round 0 instead, one sample per thread (next_n samples from epoch-local 0 into parity 0).
 __global__ void __launch_bounds__(256) bpr_det_apply_kernel(const BprParams p, const DetState d, int64_t r, int par,
-                                                            int64_t next_s0, int64_t next_n)
+                                                            int64_t next_n)
 {
     const int lane = threadIdx.x & 31;
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned int n_skipped = 0;
-    if (t < next_n) {
-        const DetPlan nx = par ? d.plan[0] : d.plan[1];
-        int64_t ii;
-        int32_t j;
-        draw_sample(p, next_s0 + t, ii, j);
-        const int2 pr = __ldg(p.pairs + ii);
-        const uint64_t key = pair_key(pr.x, j);
-        const bool skip = bucket_has(p.table, p.bucket_mask, key, mix64(key) & p.bucket_mask);    // recom_bpr.pyx:241-243
-        __stcg(nx.rec + t, make_int4(pr.x, pr.y, j, !skip));
-        if (skip) {
-            n_skipped = 1;
-        } else {
-            // the three counts first (independent round trips), then the slots of the rows that became shared
-            const unsigned cu = atomicAdd(nx.cnt_u + pr.x, 1u);
-            const unsigned ci = atomicAdd(nx.cnt_v + pr.y, 1u);
-            const unsigned cj = atomicAdd(nx.cnt_v + j, 1u);
-            unsigned int* ns = d.n_shared + (r + 1);
-            if (cu == 1u) det_share(nx.slot_u, nx.row_of_slot, ns, pr.x, (unsigned)pr.x);
-            if (ci == 1u) det_share(nx.slot_v, nx.row_of_slot, ns, pr.y, (unsigned)pr.y | DET_ITEM);
-            if (cj == 1u) det_share(nx.slot_v, nx.row_of_slot, ns, j, (unsigned)j | DET_ITEM);
-        }
+    if (r < 0) {
+        det_flush_stats(0u, det_plan(p, d.plan[0], d.n_shared, t, 0, next_n), p.stats);
+        return;
     }
-    if (r >= 0) {
-        const DetPlan pl = par ? d.plan[1] : d.plan[0];
-        const unsigned n_sh = __ldcg(d.n_shared + r);
-        const int k = p.k;
-        const unsigned n_warps = gridDim.x * (blockDim.x / 32);
-        for (unsigned s = (unsigned)(t / 32); s < n_sh; s += n_warps) {
-            const unsigned tag = __ldcg(pl.row_of_slot + s);
-            const int32_t row = (int32_t)(tag & ~DET_ITEM);
-            const bool item = tag & DET_ITEM;
-            float* x = (item ? p.V : p.U) + (size_t)row * k;
-            unsigned long long* a = d.acc + (size_t)s * (size_t)(k + 1);
-            for (int e0 = 0; e0 < k; e0 += 32 * DET_RC) {       // DET_RC elements per lane in flight at once
-                long long q[DET_RC];
-                float v[DET_RC];
+    det_pdl_sync();
+    const DetPlan pl = par ? d.plan[1] : d.plan[0];
+    const unsigned n_sh = __ldcg(d.n_shared + r);
+    const int k = p.k;
+    const unsigned n_warps = gridDim.x * (blockDim.x / 32);
+    for (unsigned s = (unsigned)(t / 32); s < n_sh; s += n_warps) {
+        const unsigned tag = __ldcg(pl.row_of_slot + s);
+        const int32_t row = (int32_t)(tag & ~DET_ITEM);
+        const bool item = tag & DET_ITEM;
+        float* x = (item ? p.V : p.U) + (size_t)row * k;
+        unsigned long long* a = d.acc + (size_t)s * (size_t)(k + 1);
+        for (int e0 = 0; e0 < k; e0 += 32 * DET_RC) {       // DET_RC elements per lane in flight at once
+            long long q[DET_RC];
+            float v[DET_RC];
 #pragma unroll
-                for (int c = 0; c < DET_RC; ++c) {
-                    const int e = e0 + lane + 32 * c;
-                    q[c] = 0;
-                    if (e < k) { q[c] = (long long)__ldcg(a + e); v[c] = __ldcg(x + e); }
-                }
-#pragma unroll
-                for (int c = 0; c < DET_RC; ++c) {
-                    const int e = e0 + lane + 32 * c;
-                    if (e < k) det_apply(a + e, x + e, q[c], v[c]);
-                }
+            for (int c = 0; c < DET_RC; ++c) {
+                const int e = e0 + lane + 32 * c;
+                q[c] = 0;
+                if (e < k) { q[c] = (long long)__ldcg(a + e); v[c] = __ldcg(x + e); }
             }
-            if (lane == 0) {
-                if (item && p.use_bias) det_apply(a + k, p.B + row, (long long)__ldcg(a + k), __ldcg(p.B + row));
-                (item ? pl.cnt_v : pl.cnt_u)[row] = 0u;
+#pragma unroll
+            for (int c = 0; c < DET_RC; ++c) {
+                const int e = e0 + lane + 32 * c;
+                if (e < k) det_apply(a + e, x + e, q[c], v[c]);
             }
         }
+        if (lane == 0) {
+            if (item && p.use_bias) det_apply(a + k, p.B + row, (long long)__ldcg(a + k), __ldcg(p.B + row));
+            (item ? pl.cnt_v : pl.cnt_u)[row] = 0u;
+        }
     }
-    det_flush_stats(0u, n_skipped, p.stats);
 }
 
 static int bpr_epoch_deterministic(const BprParams& p, int64_t n_users, cudaStream_t st)
@@ -1084,26 +1125,35 @@ static int bpr_epoch_deterministic(const BprParams& p, int64_t n_users, cudaStre
         pl.row_of_slot = ros + q * cap;
     }
     cudaError_t e = cudaMemsetAsync(buf + rec_b, 0, zero_b, st);      // every round leaves counters and slots at zero
-    // apply grid: one thread per sample of the next round's plan, and at least one resident grid of warps (capped by the
-    // slots a round can have) for the shared rows
-    const int64_t apply_min = std::min<int64_t>((int64_t)sm_count() * (2048 / 256), (cap * 32 + 255) / 256);
     auto blocks = [](int64_t threads) { return (unsigned)((threads + 255) / 256); };
+    // apply grid: one resident grid of warps for the shared rows, capped by the slots a round can have
+    const unsigned apply_grid = (unsigned)std::min<int64_t>((int64_t)sm_count() * (2048 / 256), blocks(cap * 32));
     if (e == cudaSuccess) {
-        bpr_det_apply_kernel<<<blocks(std::min(round, p.n_samples)), 256, 0, st>>>(p, d, -1, 1, 0,
-                                                                                  std::min(round, p.n_samples));
+        bpr_det_apply_kernel<<<blocks(std::min(round, p.n_samples)), 256, 0, st>>>(p, d, -1, 0, std::min(round, p.n_samples));
         ::b200::count_launch();
         e = cudaGetLastError();
     }
+    // the rounds' launches start while the launch before them runs (programmatic dependent launch, det_pdl_sync); the
+    // prologue above and whatever follows the epoch on the stream stay fully stream-ordered
+    cudaLaunchAttribute pdl;
+    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    pdl.val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(256);
+    cfg.stream = st;
+    cfg.attrs = &pdl;
+    cfg.numAttrs = 1;
     for (int64_t r = 0; r < n_rounds && e == cudaSuccess; ++r) {
         const int64_t s0 = r * round;
         const int64_t n = std::min(round, p.n_samples - s0);
         const int64_t next_n = r + 1 < n_rounds ? std::min(round, p.n_samples - s0 - round) : 0;
         const int par = (int)(r & 1);
-        bpr_det_grad_kernel<<<blocks(n * 32), 256, 0, st>>>(p, d, n, par);
-        bpr_det_apply_kernel<<<(unsigned)std::max<int64_t>(blocks(next_n), apply_min), 256, 0, st>>>(p, d, r, par,
-                                                                                                    s0 + round, next_n);
+        cfg.gridDim = dim3(blocks(next_n) + blocks(n * 32));
+        e = cudaLaunchKernelEx(&cfg, bpr_det_grad_kernel, p, d, r, par, n, s0 + round, next_n);
+        if (e != cudaSuccess) break;
+        cfg.gridDim = dim3(apply_grid);
+        e = cudaLaunchKernelEx(&cfg, bpr_det_apply_kernel, p, d, r, par, (int64_t)0);
         ::b200::count_launch(2);
-        e = cudaGetLastError();
     }
     const cudaError_t f = cudaFreeAsync(buf, st);
     if (e != cudaSuccess) return cuda_fail(e, "bpr_det_grad_kernel / bpr_det_apply_kernel", __FILE__, __LINE__);

@@ -6,7 +6,8 @@
 Builds the model with bench.py's own generator and initialisation (imported, not copied), runs W warm-up epochs, then
 one deterministic epoch under torch.profiler (CUDA activity) and writes OUTDIR/det_epoch_profile.json:
   * per kernel: total time, launch count, mean time per launch and per round (round = one bpr_det_grad_kernel launch);
-  * the gaps between consecutive kernels of the epoch (idle device time between launches);
+  * the epoch's first bpr_det_apply_kernel launch on its own: it only plans round 0, so it prices one round's plan;
+  * the gaps between consecutive kernels of the epoch (idle device time between launches) and their overlaps;
   * the epoch's span on the device, its algorithmic bytes (bench.algorithmic_bytes) and the resulting GB/s;
   * the card's name, power limit and max SM clock.
 It only calls engine.bpr_epoch(..., deterministic=True), so the same script profiles any build of the library.
@@ -96,8 +97,14 @@ def main():
     if not kev:
         raise SystemExit("det_epoch_profile.py: the trace holds no bpr_* kernel")
     n_rounds = sum(1 for e in kev if e[0] == "bpr_det_grad_kernel")
+    # the epoch's first bpr_det_apply_kernel launch applies nothing and only plans round 0: the cost of one round's plan
+    first_apply = next((x for x, e in enumerate(kev) if e[0] == "bpr_det_apply_kernel"), None)
+    prologue = None
     per = {}
-    for name, ts, dur in kev:
+    for x, (name, ts, dur) in enumerate(kev):
+        if x == first_apply:
+            prologue = {"kernel": name, "us": round(dur, 3)}
+            continue
         d = per.setdefault(name, {"count": 0, "total_us": 0.0})
         d["count"] += 1
         d["total_us"] += dur
@@ -105,8 +112,12 @@ def main():
         d["mean_us"] = round(d["total_us"] / d["count"], 3)
         d["us_per_round"] = round(d["total_us"] / max(n_rounds, 1), 3)
         d["total_us"] = round(d["total_us"], 1)
+    # a launch that starts before the one before it has ended (programmatic dependent launch) gives a negative gap: the
+    # overlap, during which the later launch may be waiting for the earlier one, so kernel times can add up to more than
+    # the span
     gaps = [kev[x + 1][1] - (kev[x][1] + kev[x][2]) for x in range(len(kev) - 1)]
     gaps_pos = [g for g in gaps if g > 0]
+    overlaps = [-g for g in gaps if g < 0]
     span_us = kev[-1][1] + kev[-1][2] - kev[0][1]
     busy_us = sum(e[2] for e in kev)
     nnz = int(data.nnz)
@@ -121,11 +132,16 @@ def main():
                   "us_per_round": round(span_us / max(n_rounds, 1), 3),
                   "algorithmic_bytes": alg, "algorithmic_gbs": round(alg / (span_us * 1e-6) / 1e9, 1)},
         "kernels": per,
+        "prologue": prologue,
         "gaps": {"count": len(gaps), "total_us": round(sum(gaps_pos), 1),
                  "mean_us": round(sum(gaps_pos) / max(len(gaps), 1), 3),
-                 "max_us": round(max(gaps) if gaps else 0.0, 3)},
+                 "max_us": round(max(gaps) if gaps else 0.0, 3),
+                 "overlaps": len(overlaps), "overlap_total_us": round(sum(overlaps), 1),
+                 "overlap_mean_us": round(sum(overlaps) / max(len(overlaps), 1), 3)},
         "note": "kernel times and gaps from torch.profiler (CUDA activity) over one epoch after %d warm-up epoch(s); "
-                "algorithmic GB/s = bench.algorithmic_bytes over the device span of the epoch's kernels" % args.warmup,
+                "`kernels` leaves out the epoch's first bpr_det_apply_kernel launch (`prologue`: the plan of round 0 "
+                "alone); algorithmic GB/s = bench.algorithmic_bytes over the device span of the epoch's kernels"
+                % args.warmup,
     }
     os.makedirs(args.outdir, exist_ok=True)
     with open(os.path.join(args.outdir, "det_epoch_profile.json"), "w") as f:
