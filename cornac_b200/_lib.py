@@ -73,6 +73,12 @@ SIGNATURES = {
     "b200_spd_inverse": (_int, [_i64, _vp, _vp, _vp, _int, _vp]),
     "b200_ease_weights": (_int, [_i64, _vp, _vp, _int, _vp]),
     "b200_ease_score": (_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200_hpf_workspace_bytes": (_i64, [_i64, _i64, _i64, _int]),
+    "b200_hpf_expect": (_int, [_vp, _vp, _i64, _vp, _vp]),
+    "b200_hpf_update": (_int, [_int, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                               _vp, _vp, _vp, _vp, _vp]),
+    "b200_hpf_fit": (_int, [_int, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                            _vp, _vp, _int, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),

@@ -1,0 +1,361 @@
+// HPF / PF (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275) for sm_90a: the coordinate-ascent variational fit in f64, in the
+// reference's update order.
+//
+// The reference is built without -ffast-math or -march, so it has no FMA and never reorders a sum.  Every product, sum
+// and quotient below is an explicitly rounded __d*_rn intrinsic in the reference's order, so given the same expectations
+// Lt / Lb an iteration is bit-identical to it.  The expectations themselves use CUDA's exp / log and a restatement of the
+// Cephes digamma, so they differ from glibc / Eigen in the last bits; the fit agrees with the reference to rounding.
+//
+// One iteration (constants a = b = 0.3; HPF: k_s = t_s = 0.3 + 0.3 g, c = 1; PF: k_s = t_s = 0.3, K_r = T_r = 1):
+//   1. hpf_expect_kernel: Lt = exp(digamma(G_s) - log(G_r)), Lb likewise; a term whose shape / rate is <= 0 is dropped
+//      and an entry with both dropped is 0 (the reference works on sparse matrices that store only positive entries);
+//   2. hpf_dk_kernel: dk = 2^-52 + sum_k Lt[u,k] Lb[i,k] for every rating, k ascending;
+//   3. hpf_pass_kernel over the CSR rows: G_s[u,k] = a + sum over the row, items ascending, of ((Lt Lb) x) / dk;
+//   4. hpf_colsum_kernel: S[k] = sum over items, ascending, of the OLD L_s / L_r (entries with L_r <= 0 skipped);
+//      hpf_rate_kernel: G_r[u,k] = k_s / K_r[u] + S[k]; HPF: K_r[u] = a / c + sum_k G_s / G_r;
+//   5. hpf_pass_kernel over the CSC columns (users ascending, dk through the CSR -> CSC map): L_s;
+//   6. S'[k] over the NEW G_s / G_r, then L_r and (HPF) T_r as in 4.
+// A skipped quotient enters the column sums as +0.0: a sum that starts at +0.0 is never -0.0, so adding +0.0 leaves it
+// unchanged bit for bit.  The column sums are one sequential chain per factor, as in the reference.
+#include "common.cuh"
+
+#include <algorithm>
+
+namespace b200 {
+
+constexpr int HPF_THREADS = 256;
+constexpr int HPF_COLSUM_UNROLL = 8;
+constexpr int HPF_PASS_BATCH = 8;
+constexpr double HPF_DK_EPS = 0x1p-52;          // pow(2, -52), cpp_hpf.cpp:43
+constexpr double HPF_A = 0.3;                   // a_ (HPF and PF)
+constexpr double HPF_B = 0.3;                   // HPF b_, PF c_: the item-side shape
+
+// psi(x) for x > 0 (the rules of step 1 never pass anything else): the recurrence psi(x) = psi(x + 1) - 1/x up to
+// s >= 10, then the asymptotic series log(s) - 1/(2s) - sum_k B_2k / (2k s^2k) with its seven Bernoulli terms in Horner
+// form, as the Cephes `psi` routine evaluates it.
+__device__ __forceinline__ double hpf_digamma(double x)
+{
+    double s = x, w = 0.0;
+    while (s < 10.0) {
+        w = __dadd_rn(w, __ddiv_rn(1.0, s));
+        s = __dadd_rn(s, 1.0);
+    }
+    double y = 0.0;
+    if (s < 1e17) {
+        const double z = __ddiv_rn(1.0, __dmul_rn(s, s));
+        double p = 1.0 / 12.0;                                  // B_14 / 14
+        p = __dadd_rn(__dmul_rn(p, z), -691.0 / 32760.0);        // B_12 / 12
+        p = __dadd_rn(__dmul_rn(p, z), 1.0 / 132.0);             // B_10 / 10
+        p = __dadd_rn(__dmul_rn(p, z), -1.0 / 240.0);            // B_8 / 8
+        p = __dadd_rn(__dmul_rn(p, z), 1.0 / 252.0);             // B_6 / 6
+        p = __dadd_rn(__dmul_rn(p, z), -1.0 / 120.0);            // B_4 / 4
+        p = __dadd_rn(__dmul_rn(p, z), 1.0 / 12.0);              // B_2 / 2
+        y = __dmul_rn(z, p);
+    }
+    return __dsub_rn(__dsub_rn(__dsub_rn(log(s), __ddiv_rn(0.5, s)), y), w);
+}
+
+// Step 1: out = exp(digamma(shape) - log(rate)) with the stored-entry rules.
+__global__ void __launch_bounds__(HPF_THREADS) hpf_expect_kernel(const double* __restrict__ shape,
+                                                                 const double* __restrict__ rate, int64_t n,
+                                                                 double* __restrict__ out)
+{
+    for (int64_t t = (int64_t)blockIdx.x * HPF_THREADS + threadIdx.x; t < n; t += (int64_t)gridDim.x * HPF_THREADS) {
+        const double s = shape[t], r = rate[t];
+        const bool hs = s > 0.0, hr = r > 0.0;
+        double v = 0.0;
+        if (hs || hr) {
+            double e = hs ? hpf_digamma(s) : 0.0;
+            if (hr) e = __dsub_rn(e, log(r));
+            v = exp(e);
+        }
+        out[t] = v;
+    }
+}
+
+// Q = R > 0 ? S / R : +0.0, the quotients the column sums add.
+__global__ void __launch_bounds__(HPF_THREADS) hpf_quotient_kernel(const double* __restrict__ S,
+                                                                   const double* __restrict__ R, int64_t n,
+                                                                   double* __restrict__ Q)
+{
+    for (int64_t t = (int64_t)blockIdx.x * HPF_THREADS + threadIdx.x; t < n; t += (int64_t)gridDim.x * HPF_THREADS) {
+        const double r = R[t];
+        Q[t] = r > 0.0 ? __ddiv_rn(S[t], r) : 0.0;
+    }
+}
+
+// Step 2: a thread per rating (CSR order).
+__global__ void __launch_bounds__(HPF_THREADS) hpf_dk_kernel(const int32_t* __restrict__ row,
+                                                             const int32_t* __restrict__ col, int64_t nnz, int k,
+                                                             const double* __restrict__ Lt,
+                                                             const double* __restrict__ Lb, double* __restrict__ dk)
+{
+    for (int64_t j = (int64_t)blockIdx.x * HPF_THREADS + threadIdx.x; j < nnz; j += (int64_t)gridDim.x * HPF_THREADS) {
+        const double* a = Lt + (size_t)__ldg(row + j) * k;
+        const double* b = Lb + (size_t)__ldg(col + j) * k;
+        double d = HPF_DK_EPS;
+        for (int f = 0; f < k; ++f) d = __dadd_rn(d, __dmul_rn(__ldg(a + f), __ldg(b + f)));
+        dk[j] = d;
+    }
+}
+
+// Steps 3 and 5: a thread per (row, factor) of the side being updated.  Row r's entries are [ptr[r], ptr[r+1]); entry c
+// pairs r with row oid[c] of the other side, has rating val[c] and its dk at dk[pos ? pos[c] : c].  USER_SIDE: the
+// product is own[r,f] * other[o,f] (Lt * Lb); otherwise other[o,f] * own[r,f] (again Lt * Lb).
+template <bool USER_SIDE>
+__global__ void __launch_bounds__(HPF_THREADS) hpf_pass_kernel(const int32_t* __restrict__ ptr,
+                                                               const int32_t* __restrict__ oid,
+                                                               const double* __restrict__ val,
+                                                               const int32_t* __restrict__ pos,
+                                                               const double* __restrict__ dk, int64_t n_rows, int k,
+                                                               const double* __restrict__ own,
+                                                               const double* __restrict__ other, double shape0,
+                                                               double* __restrict__ out)
+{
+    const int64_t n = n_rows * k;
+    for (int64_t t = (int64_t)blockIdx.x * HPF_THREADS + threadIdx.x; t < n; t += (int64_t)gridDim.x * HPF_THREADS) {
+        const int64_t r = t / k;
+        const int f = (int)(t - r * k);
+        const double e = __ldg(own + t);
+        const int32_t lo = __ldg(ptr + r), hi = __ldg(ptr + r + 1);
+        auto term = [&](double o, double x, double d) {
+            const double p = USER_SIDE ? __dmul_rn(e, o) : __dmul_rn(o, e);
+            return __ddiv_rn(__dmul_rn(p, x), d);
+        };
+        double acc = shape0;
+        int32_t c = lo;
+        // the gathers of HPF_PASS_BATCH entries are issued together (the division's slow path is a call the compiler
+        // does not schedule loads across), then the terms are added in entry order
+        for (; c + HPF_PASS_BATCH <= hi; c += HPF_PASS_BATCH) {
+            double o[HPF_PASS_BATCH], x[HPF_PASS_BATCH], d[HPF_PASS_BATCH];
+#pragma unroll
+            for (int q = 0; q < HPF_PASS_BATCH; ++q) {
+                o[q] = __ldg(other + (size_t)__ldg(oid + c + q) * k + f);
+                x[q] = __ldg(val + c + q);
+                d[q] = __ldg(dk + (pos ? __ldg(pos + c + q) : c + q));
+            }
+#pragma unroll
+            for (int q = 0; q < HPF_PASS_BATCH; ++q) acc = __dadd_rn(acc, term(o[q], x[q], d[q]));
+        }
+        for (; c < hi; ++c)
+            acc = __dadd_rn(acc, term(__ldg(other + (size_t)__ldg(oid + c) * k + f), __ldg(val + c),
+                                      __ldg(dk + (pos ? __ldg(pos + c) : c))));
+        out[t] = acc;
+    }
+}
+
+// Steps 4 and 6, the column sums: a thread per factor, one sequential chain over the rows.  The loads run ahead of the
+// chain in groups of HPF_COLSUM_UNROLL rows; the adds stay in row order.
+__global__ void __launch_bounds__(32) hpf_colsum_kernel(const double* __restrict__ Q, int64_t n_rows, int k,
+                                                        double* __restrict__ out)
+{
+    const int f = blockIdx.x * 32 + threadIdx.x;
+    if (f >= k) return;
+    double acc = 0.0;
+    int64_t r = 0;
+    for (; r + HPF_COLSUM_UNROLL <= n_rows; r += HPF_COLSUM_UNROLL) {
+        double q[HPF_COLSUM_UNROLL];
+#pragma unroll
+        for (int u = 0; u < HPF_COLSUM_UNROLL; ++u) q[u] = __ldg(Q + (size_t)(r + u) * k + f);
+#pragma unroll
+        for (int u = 0; u < HPF_COLSUM_UNROLL; ++u) acc = __dadd_rn(acc, q[u]);
+    }
+    for (; r < n_rows; ++r) acc = __dadd_rn(acc, __ldg(Q + (size_t)r * k + f));
+    out[f] = acc;
+}
+
+// Steps 4 and 6, the row updates: a thread per row.  RATE: R[r,f] = shape_s / Kr[r] + colsum[f].  KAPPA: Kr[r] = a/c +
+// sum_f S[r,f] / R[r,f] (f ascending, nothing skipped: update_kappa_r).  Q (may be NULL): the quotients the next column
+// sum adds, R > 0 ? S / R : +0.0.
+template <bool RATE, bool KAPPA>
+__global__ void __launch_bounds__(HPF_THREADS) hpf_rate_kernel(int64_t n_rows, int k, const double* __restrict__ S,
+                                                               double* __restrict__ R, double* __restrict__ Kr,
+                                                               const double* __restrict__ colsum, double shape_s,
+                                                               double a_over_c, double* __restrict__ Q)
+{
+    for (int64_t r = (int64_t)blockIdx.x * HPF_THREADS + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * HPF_THREADS) {
+        const size_t base = (size_t)r * k;
+        if constexpr (RATE) {
+            const double head = __ddiv_rn(shape_s, Kr[r]);
+            for (int f = 0; f < k; ++f) R[base + f] = __dadd_rn(head, __ldg(colsum + f));
+        }
+        double sum = 0.0;
+        for (int f = 0; f < k; ++f) {
+            const double rv = R[base + f];
+            const double q = __ddiv_rn(__ldg(S + base + f), rv);
+            if constexpr (KAPPA) sum = __dadd_rn(sum, q);
+            if (Q) Q[base + f] = rv > 0.0 ? q : 0.0;
+        }
+        if constexpr (KAPPA) Kr[r] = __dadd_rn(a_over_c, sum);
+    }
+}
+
+unsigned hpf_grid(int64_t n)
+{
+    const int64_t cap = (int64_t)sm_count() * 16;
+    return (unsigned)std::max<int64_t>(1, std::min<int64_t>(cap, (n + HPF_THREADS - 1) / HPF_THREADS));
+}
+
+struct HpfWork {
+    double *dk, *qL, *qG, *S, *S2, *Lt, *Lb;
+};
+
+HpfWork hpf_carve(double* w, int64_t n_users, int64_t n_items, int64_t nnz, int k)
+{
+    HpfWork h;
+    h.dk = w;
+    h.qL = h.dk + std::max<int64_t>(nnz, 1);
+    h.qG = h.qL + n_items * k;
+    h.S = h.qG + n_users * k;
+    h.S2 = h.S + k;
+    h.Lt = h.S2 + k;
+    h.Lb = h.Lt + n_users * k;
+    return h;
+}
+
+void hpf_expect(const double* shape, const double* rate, int64_t n, double* out, cudaStream_t st)
+{
+    if (n == 0) return;
+    hpf_expect_kernel<<<hpf_grid(n), HPF_THREADS, 0, st>>>(shape, rate, n, out);
+    count_launch();
+}
+
+template <bool RATE, bool KAPPA>
+void hpf_rate(int64_t n_rows, int k, const double* S, double* R, double* Kr, const double* colsum, double shape_s,
+              double a_over_c, double* Q, cudaStream_t st)
+{
+    if (n_rows == 0) return;
+    hpf_rate_kernel<RATE, KAPPA><<<hpf_grid(n_rows), HPF_THREADS, 0, st>>>(n_rows, k, S, R, Kr, colsum, shape_s,
+                                                                          a_over_c, Q);
+    count_launch();
+}
+
+struct HpfArgs {
+    int hierarchical;
+    int64_t n_users, n_items, nnz;
+    int k;
+    const int32_t *indptr, *indices, *row;
+    const double* val;
+    const int32_t *csc_ptr, *csc_row, *csc_pos;
+    const double* csc_val;
+    double *Gs, *Gr, *Ls, *Lr, *Kr, *Tr;
+};
+
+// Steps 2-6 of one iteration from the expectations Lt, Lb.
+void hpf_update(const HpfArgs& a, const double* Lt, const double* Lb, const HpfWork& w, cudaStream_t st)
+{
+    const int k = a.k;
+    const double ks = a.hierarchical ? HPF_A + (double)k * HPF_A : HPF_A;
+    const double ts = a.hierarchical ? HPF_B + (double)k * HPF_B : HPF_B;
+    const double c = 1.0;
+    const unsigned gk = (unsigned)((k + 31) / 32);
+    // S from the old L_s / L_r (update_gamma_r before update_lambda_s)
+    if (a.n_items * k > 0) {
+        hpf_quotient_kernel<<<hpf_grid(a.n_items * k), HPF_THREADS, 0, st>>>(a.Ls, a.Lr, a.n_items * k, w.qL);
+        count_launch();
+    }
+    hpf_colsum_kernel<<<gk, 32, 0, st>>>(w.qL, a.n_items, k, w.S);
+    count_launch();
+    if (a.nnz > 0) {
+        hpf_dk_kernel<<<hpf_grid(a.nnz), HPF_THREADS, 0, st>>>(a.row, a.indices, a.nnz, k, Lt, Lb, w.dk);
+        count_launch();
+    }
+    if (a.n_users > 0) {
+        hpf_pass_kernel<true><<<hpf_grid(a.n_users * k), HPF_THREADS, 0, st>>>(
+            a.indptr, a.indices, a.val, nullptr, w.dk, a.n_users, k, Lt, Lb, HPF_A, a.Gs);
+        count_launch();
+    }
+    if (a.hierarchical)
+        hpf_rate<true, true>(a.n_users, k, a.Gs, a.Gr, a.Kr, w.S, ks, HPF_A / c, w.qG, st);
+    else
+        hpf_rate<true, false>(a.n_users, k, a.Gs, a.Gr, a.Kr, w.S, ks, 0.0, w.qG, st);
+    hpf_colsum_kernel<<<gk, 32, 0, st>>>(w.qG, a.n_users, k, w.S2);
+    count_launch();
+    if (a.n_items > 0) {
+        hpf_pass_kernel<false><<<hpf_grid(a.n_items * k), HPF_THREADS, 0, st>>>(
+            a.csc_ptr, a.csc_row, a.csc_val, a.csc_pos, w.dk, a.n_items, k, Lb, Lt, HPF_B, a.Ls);
+        count_launch();
+    }
+    if (a.hierarchical)
+        hpf_rate<true, true>(a.n_items, k, a.Ls, a.Lr, a.Tr, w.S2, ts, HPF_B / c, nullptr, st);
+    else
+        hpf_rate<true, false>(a.n_items, k, a.Ls, a.Lr, a.Tr, w.S2, ts, 0.0, nullptr, st);
+}
+
+int hpf_check(const HpfArgs& a, const void* work, const char* what)
+{
+    B200_REQUIRE(a.k >= 1 && a.n_users >= 0 && a.n_items >= 0 && a.nnz >= 0 && a.nnz < (1ll << 31) &&
+                     a.n_users < (1ll << 31) && a.n_items < (1ll << 31),
+                 "%s: bad sizes k=%d n_users=%lld n_items=%lld nnz=%lld", what, a.k, (long long)a.n_users,
+                 (long long)a.n_items, (long long)a.nnz);
+    B200_REQUIRE(a.indptr && a.csc_ptr && work && (a.n_users == 0 || (a.Gs && a.Gr && a.Kr)) &&
+                     (a.n_items == 0 || (a.Ls && a.Lr && a.Tr)),
+                 "%s: null pointer argument", what);
+    B200_REQUIRE(a.nnz == 0 || (a.indices && a.row && a.val && a.csc_row && a.csc_pos && a.csc_val),
+                 "%s: null rating arrays", what);
+    return B200_OK;
+}
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" int64_t b200_hpf_workspace_bytes(int64_t n_users, int64_t n_items, int64_t nnz, int k)
+{
+    if (n_users < 0 || n_items < 0 || nnz < 0 || k < 1) return -1;
+    return (int64_t)sizeof(double) * (std::max<int64_t>(nnz, 1) + 2 * (n_users + n_items) * k + 2 * (int64_t)k);
+}
+
+extern "C" int b200_hpf_expect(const double* shape, const double* rate, int64_t n, double* out, void* stream)
+{
+    B200_REQUIRE(n >= 0, "b200_hpf_expect: bad size n=%lld", (long long)n);
+    B200_REQUIRE(n == 0 || (shape && rate && out), "b200_hpf_expect: null pointer argument");
+    hpf_expect(shape, rate, n, out, (cudaStream_t)stream);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+
+#define B200_HPF_ARGS                                                                                                  \
+    HpfArgs a{hierarchical, n_users, n_items, nnz, k, indptr, indices, row, val, csc_ptr, csc_row, csc_pos, csc_val,   \
+              Gs, Gr, Ls, Lr, Kr, Tr}
+
+extern "C" int b200_hpf_update(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k,
+                               const int32_t* indptr, const int32_t* indices, const int32_t* row, const double* val,
+                               const int32_t* csc_ptr, const int32_t* csc_row, const int32_t* csc_pos,
+                               const double* csc_val, const double* Lt, const double* Lb, double* Gs, double* Gr,
+                               double* Ls, double* Lr, double* Kr, double* Tr, double* work, void* stream)
+{
+    B200_HPF_ARGS;
+    if (int rc = hpf_check(a, work, "b200_hpf_update")) return rc;
+    B200_REQUIRE((n_users == 0 || Lt) && (n_items == 0 || Lb), "b200_hpf_update: null Lt / Lb");
+    hpf_update(a, Lt, Lb, hpf_carve(work, n_users, n_items, nnz, k), (cudaStream_t)stream);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+
+extern "C" int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k,
+                            const int32_t* indptr, const int32_t* indices, const int32_t* row, const double* val,
+                            const int32_t* csc_ptr, const int32_t* csc_row, const int32_t* csc_pos,
+                            const double* csc_val, double* Gs, double* Gr, double* Ls, double* Lr, double* Kr,
+                            double* Tr, int max_iter, double* work, void* stream)
+{
+    B200_HPF_ARGS;
+    if (int rc = hpf_check(a, work, "b200_hpf_fit")) return rc;
+    B200_REQUIRE(max_iter >= 0, "b200_hpf_fit: bad max_iter=%d", max_iter);
+    cudaStream_t st = (cudaStream_t)stream;
+    const HpfWork w = hpf_carve(work, n_users, n_items, nnz, k);
+    // hpf_cpp's update_kappa_r before the loop.  After an iteration K_r and T_r already hold these values, so a fit split
+    // into several calls recomputes them bit for bit.
+    if (hierarchical) {
+        hpf_rate<false, true>(n_users, k, Gs, Gr, Kr, nullptr, 0.0, HPF_A / 1.0, nullptr, st);
+        hpf_rate<false, true>(n_items, k, Ls, Lr, Tr, nullptr, 0.0, HPF_B / 1.0, nullptr, st);
+    }
+    for (int it = 0; it < max_iter; ++it) {
+        hpf_expect(Gs, Gr, n_users * k, w.Lt, st);
+        hpf_expect(Ls, Lr, n_items * k, w.Lb, st);
+        hpf_update(a, w.Lt, w.Lb, w, st);
+    }
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+#undef B200_HPF_ARGS

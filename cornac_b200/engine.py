@@ -12,6 +12,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     score_batch_f64 / topk_rows_f64 <-> PMF.score / Recommender.rank (cornac/models/pmf/recom_pmf.py:191-222)
     nmf_prepare / nmf_fit          <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
     ease_fit / ease_score          <-> EASE.fit / EASE.score (cornac/models/ease/recom_ease.py:57-126)
+    hpf_fit / hpf_update / hpf_expect <-> hpf_cpp / pf_cpp   (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275)
 """
 import numpy as np
 import scipy.sparse as _sp
@@ -921,6 +922,113 @@ def nmf_fit(data, U, V, Bu, Bi, n_epochs, mu=0.0, learning_rate=0.005, lambda_u=
                          data.n_levels, k, ptr(U), ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs),
                          f32(mu), f32(learning_rate), f32(lambda_u), f32(lambda_v), f32(lambda_bu), f32(lambda_bi),
                          int(data.use_bias), ptr(loss), current_stream()), "b200_nmf_fit")
+
+
+class HpfData:
+    """Device copy of HPF's ratings, built once per fit and used by every iteration: the CSR (indptr, items, f64 values,
+    and each entry's user) and its CSC transpose (users ascending in each column) with the CSR index of each entry.
+    rid, cid, val: the stored (user, item, value) triplets, each pair at most once; zeros are the caller's to drop."""
+
+    def __init__(self, rid, cid, val, n_users, n_items):
+        require_cuda()
+        rid = np.asarray(rid, dtype=np.int64)
+        cid = np.asarray(cid, dtype=np.int64)
+        val = np.asarray(val, dtype=np.float64)
+        self.n_users, self.n_items, self.nnz = int(n_users), int(n_items), len(rid)
+        if len(cid) != self.nnz or len(val) != self.nnz:
+            raise B200Error("rid, cid and val differ in length (%d, %d, %d)" % (self.nnz, len(cid), len(val)))
+        if self.nnz >= 2 ** 31:
+            raise B200Error("nnz >= 2^31 is not supported (int32 offsets)")
+        if self.nnz and (rid.min() < 0 or rid.max() >= self.n_users or cid.min() < 0 or cid.max() >= self.n_items):
+            raise B200Error("a rating lies outside the %d x %d matrix" % (self.n_users, self.n_items))
+        order = np.lexsort((cid, rid))                       # CSR: users, then items ascending
+        rid, cid, val = rid[order], cid[order], val[order]
+        if self.nnz > 1 and np.any((rid[1:] == rid[:-1]) & (cid[1:] == cid[:-1])):
+            raise B200Error("a (user, item) pair is stored twice")
+        indptr = np.zeros(self.n_users + 1, dtype=np.int64)
+        np.cumsum(np.bincount(rid, minlength=self.n_users), out=indptr[1:])
+        csc_ptr, csc_pos, _ = nmf_prepare(indptr.astype(np.int32), cid.astype(np.int32), self.n_items)
+        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
+        self.indptr = to_device(indptr.astype(np.int32), torch.int32)
+        self.indices = to_device(pad(cid.astype(np.int32)), torch.int32)
+        self.row = to_device(pad(rid.astype(np.int32)), torch.int32)
+        self.val = to_device(pad(val), torch.float64)
+        self.csc_ptr = to_device(csc_ptr, torch.int32)
+        self.csc_pos = to_device(pad(csc_pos), torch.int32)
+        self.csc_row = to_device(pad(rid[csc_pos].astype(np.int32)), torch.int32)
+        self.csc_val = to_device(pad(val[csc_pos]), torch.float64)
+        self._work = {}
+
+    def workspace(self, k):
+        """The device scratch of b200_hpf_fit / b200_hpf_update for k factors, allocated once per k."""
+        if k not in self._work:
+            nbytes = _lib.load().b200_hpf_workspace_bytes(self.n_users, self.n_items, self.nnz, int(k))
+            if nbytes < 0:
+                raise B200Error("bad HPF sizes")
+            self._work = {k: torch.empty(nbytes // 8, dtype=torch.float64, device="cuda")}
+        return self._work[k]
+
+    def args(self):
+        return (self.n_users, self.n_items, self.nnz)
+
+    def arrays(self):
+        return (ptr(self.indptr), ptr(self.indices), ptr(self.row), ptr(self.val), ptr(self.csc_ptr), ptr(self.csc_row),
+                ptr(self.csc_pos), ptr(self.csc_val))
+
+
+def _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr):
+    k = int(Gs.shape[1]) if Gs.dim() == 2 else 0
+    for t, name, rows in ((Gs, "Gs", data.n_users), (Gr, "Gr", data.n_users), (Ls, "Ls", data.n_items),
+                          (Lr, "Lr", data.n_items)):
+        _dev(t, torch.float64, name)
+        if t.dim() != 2 or int(t.shape[0]) != rows or int(t.shape[1]) != k or k < 1:
+            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, max(k, 1), tuple(t.shape)))
+    for t, name, rows in ((Kr, "Kr", data.n_users), (Tr, "Tr", data.n_items)):
+        _dev(t, torch.float64, name)
+        if t.numel() != rows:
+            raise B200Error("%s must hold %d values, got %d" % (name, rows, t.numel()))
+    return k
+
+
+def hpf_fit(data, hierarchical, Gs, Gr, Ls, Lr, Kr, Tr, max_iter):
+    """max_iter iterations of hpf_cpp (hierarchical) or pf_cpp (cpp_hpf.cpp:139-275) over `data` (HpfData), updating the
+    f64 device tensors Gs, Gr [n_users, k], Ls, Lr [n_items, k], Kr [n_users], Tr [n_items] in place.  Two calls of a and
+    b iterations equal one call of a + b."""
+    L = require_cuda()
+    k = _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr)
+    if int(max_iter) < 0:
+        raise B200Error("max_iter must be >= 0, got %d" % int(max_iter))
+    check(L.b200_hpf_fit(int(bool(hierarchical)), *data.args(), k, *data.arrays(), ptr(Gs), ptr(Gr), ptr(Ls), ptr(Lr),
+                         ptr(Kr), ptr(Tr), int(max_iter), ptr(data.workspace(k)), current_stream()), "b200_hpf_fit")
+
+
+def hpf_update(data, hierarchical, Lt, Lb, Gs, Gr, Ls, Lr, Kr, Tr):
+    """One iteration of the fit from given expectations Lt [n_users, k] and Lb [n_items, k] (f64 device tensors)."""
+    L = require_cuda()
+    k = _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr)
+    for t, name, rows in ((Lt, "Lt", data.n_users), (Lb, "Lb", data.n_items)):
+        _dev(t, torch.float64, name)
+        if tuple(t.shape) != (rows, k):
+            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, k, tuple(t.shape)))
+    check(L.b200_hpf_update(int(bool(hierarchical)), *data.args(), k, *data.arrays(), ptr(Lt), ptr(Lb), ptr(Gs), ptr(Gr),
+                            ptr(Ls), ptr(Lr), ptr(Kr), ptr(Tr), ptr(data.workspace(k)), current_stream()),
+          "b200_hpf_update")
+
+
+def hpf_expect(shape, rate, out=None):
+    """exp(digamma(shape) - log(rate)) element-wise on f64 device tensors, with HPF's stored-entry rules: a term whose
+    argument is <= 0 is dropped, and an entry with both dropped is 0."""
+    L = require_cuda()
+    _dev(shape, torch.float64, "shape"), _dev(rate, torch.float64, "rate")
+    if shape.shape != rate.shape:
+        raise B200Error("shape and rate differ in shape: %s, %s" % (tuple(shape.shape), tuple(rate.shape)))
+    if out is None:
+        out = torch.empty_like(shape)
+    _dev(out, torch.float64, "out")
+    if out.shape != shape.shape:
+        raise B200Error("out must have shape %s" % (tuple(shape.shape),))
+    check(L.b200_hpf_expect(ptr(shape), ptr(rate), shape.numel(), ptr(out), current_stream()), "b200_hpf_expect")
+    return out
 
 
 def rank_pack_items(V, item_base=None, n_items=None):

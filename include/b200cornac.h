@@ -375,6 +375,39 @@ B200_API int b200_ease_score(const int64_t* users, int64_t n_q, int64_t n_items,
                              const int32_t* indices, const double* data, const double* B, double* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * HPF / PF (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275): the variational fit of (hierarchical) Poisson factorisation in
+ * f64, in the reference's update order.  hierarchical != 0 is hpf_cpp (K_r and T_r updated), 0 is pf_cpp (they stay).
+ * Every product, sum and quotient of the update is rounded on its own (no FMA) in the reference's order, so
+ * b200_hpf_update is a fixed function of its inputs; the expectations use CUDA's exp / log and a Cephes digamma.
+ *
+ * The ratings (n_users x n_items, nnz stored values, no explicit zeros):
+ *   indptr, indices, val     device CSR int32[n_users + 1] / int32[nnz] / f64[nnz], items ascending in each row
+ *   row                      device int32[nnz]: the user of each CSR entry
+ *   csc_ptr, csc_row, csc_pos, csc_val   device CSC int32[n_items + 1] / int32[nnz] / int32[nnz] / f64[nnz], users
+ *                            ascending in each column; csc_pos = the CSR index of each CSC entry
+ * The state, device f64, updated in place: Gs, Gr [n_users, k]; Ls, Lr [n_items, k]; Kr [n_users]; Tr [n_items].
+ * work: device scratch of b200_hpf_workspace_bytes(n_users, n_items, nnz, k) bytes.
+ *
+ * b200_hpf_expect: out[t] = exp(digamma(shape[t]) - log(rate[t])), where a term whose argument is <= 0 (or NaN) is
+ *   dropped, and out[t] = 0 when both are: the reference's sparse expectation matrices store positive entries only.
+ * b200_hpf_update: one iteration from given expectations Lt [n_users, k] and Lb [n_items, k] (device f64): G_s, G_r,
+ *   (HPF) K_r, then L_s, L_r, (HPF) T_r.
+ * b200_hpf_fit: max_iter iterations (expectations + update), enqueued without a host synchronisation.  With
+ *   hierarchical it first sets K_r and T_r from the state, as hpf_cpp does before its loop; those are the values an
+ *   iteration leaves, so two calls of a and b iterations equal one call of a + b.                                       */
+B200_API int64_t b200_hpf_workspace_bytes(int64_t n_users, int64_t n_items, int64_t nnz, int k);
+B200_API int b200_hpf_expect(const double* shape, const double* rate, int64_t n, double* out, void* stream);
+B200_API int b200_hpf_update(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k, const int32_t* indptr,
+                             const int32_t* indices, const int32_t* row, const double* val, const int32_t* csc_ptr,
+                             const int32_t* csc_row, const int32_t* csc_pos, const double* csc_val, const double* Lt,
+                             const double* Lb, double* Gs, double* Gr, double* Ls, double* Lr, double* Kr, double* Tr,
+                             double* work, void* stream);
+B200_API int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k, const int32_t* indptr,
+                          const int32_t* indices, const int32_t* row, const double* val, const int32_t* csc_ptr,
+                          const int32_t* csc_row, const int32_t* csc_pos, const double* csc_val, double* Gs, double* Gr,
+                          double* Ls, double* Lr, double* Kr, double* Tr, int max_iter, double* work, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
