@@ -1,6 +1,7 @@
 """cornac_b200 -- H100 (sm_90a) implementation of Cornac's BPR / MF train-and-rank hot path.
 
     from cornac_b200 import BPR, MF, PMF, NMF   # drop-in for cornac.models.BPR / MF / PMF / NMF
+    from cornac_b200 import SoRec, MCF          # ... and the graph co-factorisations cornac.models.SoRec / MCF
     cornac.Experiment(eval_method=..., models=[BPR(k=64, ...)], metrics=[...]).run()
 
 Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b200.engine
@@ -8,7 +9,7 @@ Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b
 plug-ins).  The plug-in classes need the `cornac` package importable (they subclass its
 Recommender so that cornac.Experiment accepts them); the engine does not.
 """
-__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "HPF", "engine", "B200Error"]
+__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "HPF", "SoRec", "MCF", "engine", "B200Error"]
 
 from ._lib import B200Error  # noqa: F401
 
@@ -50,6 +51,12 @@ def __getattr__(name):
     if name == "HPF":
         from .recom_hpf import HPF
         return HPF
+    if name == "SoRec":
+        from .recom_sorec import SoRec
+        return SoRec
+    if name == "MCF":
+        from .recom_mcf import MCF
+        return MCF
     if name == "BaselineOnly":
         from .recom_bo import BaselineOnly
         return BaselineOnly

@@ -64,6 +64,9 @@ SIGNATURES = {
     "b200_pmf_fit": (_int, [_int, _vp, _vp, _vp, _vp, _i32, _i64, _int, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _vp,
                             _vp, _vp]),
     "b200_pmf_sigmoid": (_int, [_vp, _i64, _vp, _vp]),
+    "b200_cofactor_schedule": (_int, [_int, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
+    "b200_cofactor_fit": (_int, [_int, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _int,
+                                 _f32, _f32, _f32, _f32, _vp, _vp, _vp]),
     "b200_nmf_prepare": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200_nmf_fit": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _int,
                             _vp, _vp, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _f32, _f32, _f32, _int, _vp, _vp]),
@@ -111,6 +114,7 @@ BPR_LOSS_HINGE = 16
 BPR_BLOCKED = 32
 BPR_DETERMINISTIC = 64
 PMF_LINEAR, PMF_NON_LINEAR = 0, 1
+COFACTOR_SOREC, COFACTOR_MCF = 0, 1
 SPD_POTRF, SPD_TRTRI, SPD_LAUUM, SPD_ALL = 1, 2, 4, 7
 METRIC_NDCG, METRIC_PRECISION, METRIC_RECALL, METRIC_FMEASURE, METRIC_HIT, METRIC_NCRR = range(6)
 

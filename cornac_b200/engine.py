@@ -9,6 +9,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     topk_rows / rank_topk          <-> Recommender.rank      (cornac/models/recommender.py:476-530)
     knn_similarity / knn_score     <-> compute_similarity / compute_score (cornac/models/knn/similarity.pyx)
     pmf_schedule / pmf_fit         <-> pmf_linear / pmf_non_linear (cornac/models/pmf/cython/pmf.pyx:55-173)
+    cofactor_schedule / cofactor_fit <-> sorec / mcf (cornac/models/sorec/cython/sorec.pyx, cornac/models/mcf/cython/mcf.pyx)
     score_batch_f64 / topk_rows_f64 <-> PMF.score / Recommender.rank (cornac/models/pmf/recom_pmf.py:191-222)
     nmf_prepare / nmf_fit          <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
     ease_fit / ease_score          <-> EASE.fit / EASE.score (cornac/models/ease/recom_ease.py:57-126)
@@ -831,6 +832,79 @@ def pmf_sigmoid(z):
     out = torch.empty_like(z)
     check(L.b200_pmf_sigmoid(ptr(z), z.numel(), ptr(out), current_stream()), "b200_pmf_sigmoid")
     return out
+
+
+COFACTOR_VARIANTS = {"sorec": _lib.COFACTOR_SOREC, "mcf": _lib.COFACTOR_MCF}
+
+
+def cofactor_schedule(variant, net_a, net_b, uid, iid, n_users, n_items):
+    """Level schedule of a SoRec / MCF epoch (host, no device needed): the n_edges graph edges (net_a, net_b: user ids for
+    "sorec", item ids for "mcf") then the ratings (uid, iid), one stream.  Returns (order int32 [n_edges + n_ratings],
+    level_ptr int32 [n_levels + 1]); order holds stored indices, edge e at e and rating r at n_edges + r.  The updates of
+    one level touch pairwise disjoint rows of U, V and Z, and inside a level the slots keep the stored order."""
+    L = _lib.load()
+    if variant not in COFACTOR_VARIANTS:
+        raise B200Error('variant must be one of {"sorec","mcf"}, got %r' % (variant,))
+    net_a, net_b, uid, iid = (np.ascontiguousarray(x, dtype=np.int32) for x in (net_a, net_b, uid, iid))
+    if len(net_b) != len(net_a) or len(iid) != len(uid):
+        raise B200Error("edge ids (%d, %d) or rating ids (%d, %d) differ in length"
+                        % (len(net_a), len(net_b), len(uid), len(iid)))
+    n = len(net_a) + len(uid)
+    order = np.empty(n, dtype=np.int32)
+    level_ptr = np.empty(n + 1, dtype=np.int32)
+    n_levels = np.zeros(1, dtype=np.int32)
+    check(L.b200_cofactor_schedule(COFACTOR_VARIANTS[variant], ptr(net_a), ptr(net_b), len(net_a), ptr(uid), ptr(iid),
+                                   len(uid), int(n_users), int(n_items), ptr(order), ptr(level_ptr), ptr(n_levels)),
+          "b200_cofactor_schedule")
+    return order, level_ptr[: int(n_levels[0]) + 1].copy()
+
+
+class CofactorData:
+    """Device copy of a SoRec / MCF epoch in schedule order (b200_cofactor_schedule), built once per fit and used by
+    every epoch: per slot the two row ids, the target (edge value or rating) and whether it is an edge."""
+
+    def __init__(self, variant, net_a, net_b, net_val, uid, iid, rat, n_users, n_items):
+        require_cuda()
+        self.variant = variant
+        self.n_edges, self.n_ratings = len(net_a), len(uid)
+        if len(net_val) != self.n_edges or len(rat) != self.n_ratings:
+            raise B200Error("net_val has %d values for %d edges, rat %d for %d ratings"
+                            % (len(net_val), self.n_edges, len(rat), self.n_ratings))
+        self.order_host, level_ptr = cofactor_schedule(variant, net_a, net_b, uid, iid, n_users, n_items)
+        self.n_levels = len(level_ptr) - 1
+        o = self.order_host
+        cat = lambda x, y, t: np.concatenate([np.asarray(x, dtype=t), np.asarray(y, dtype=t)])[o]   # noqa: E731
+        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)                                        # noqa: E731
+        self.a_id = to_device(pad(cat(net_a, uid, np.int32)), torch.int32)
+        self.b_id = to_device(pad(cat(net_b, iid, np.int32)), torch.int32)
+        self.val = to_device(pad(cat(net_val, rat, np.float32)), torch.float32)
+        self.is_edge = to_device(pad((o < self.n_edges).astype(np.uint8)), torch.uint8)
+        self.level_ptr = to_device(level_ptr, torch.int32)
+        self.order = to_device(pad(o), torch.int32)
+
+
+def cofactor_fit(data, U, V, Z, cache_u, cache_v, cache_z, n_epochs, lambda_c, lambda_reg, learning_rate, gamma,
+                 loss=None):
+    """n_epochs epochs of sorec / mcf (sorec.pyx:78-143, mcf.pyx:80-144) over `data` (CofactorData), updating the f64
+    device tensors U, V, Z and their RMSProp caches in place.  lambda_c is used by SoRec only; the hyperparameters are
+    the reference's C floats.  loss: optional f64 device tensor [n_epochs, n_edges + n_ratings] that receives each
+    update's loss term at its stored index."""
+    L = require_cuda()
+    k = int(U.shape[1])
+    for t, name in ((U, "U"), (V, "V"), (Z, "Z"), (cache_u, "cache_u"), (cache_v, "cache_v"), (cache_z, "cache_z")):
+        _dev(t, torch.float64, name)
+        if t.dim() != 2 or int(t.shape[1]) != k:
+            raise B200Error("%s must be 2-D with %d columns" % (name, k))
+    n_total = data.n_edges + data.n_ratings
+    if loss is not None:
+        _dev(loss, torch.float64, "loss")
+        if loss.numel() != int(n_epochs) * n_total:
+            raise B200Error("loss must hold n_epochs * (n_edges + n_ratings) = %d values" % (int(n_epochs) * n_total))
+    check(L.b200_cofactor_fit(COFACTOR_VARIANTS[data.variant], ptr(data.a_id), ptr(data.b_id), ptr(data.val),
+                              ptr(data.is_edge), ptr(data.level_ptr), data.n_levels, data.n_edges, data.n_ratings, k,
+                              ptr(U), ptr(V), ptr(Z), ptr(cache_u), ptr(cache_v), ptr(cache_z), int(n_epochs),
+                              float(lambda_c), float(lambda_reg), float(learning_rate), float(gamma), ptr(loss),
+                              ptr(data.order) if loss is not None else None, current_stream()), "b200_cofactor_fit")
 
 
 def nmf_prepare(indptr, indices, n_items):

@@ -301,6 +301,43 @@ B200_API int b200_pmf_fit(int variant, const int32_t* uid, const int32_t* iid, c
 B200_API int b200_pmf_sigmoid(const float* z, int64_t n, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * SoRec (cornac/models/sorec/cython/sorec.pyx:40-147) and MCF (cornac/models/mcf/cython/mcf.pyx:43-148): per epoch
+ * the non-linear PMF update (pmf_non_linear's element steps, in f64) over the n_edges graph edges in stored order, then
+ * over the n_ratings ratings.  The epoch is one stream of n_edges + n_ratings updates (edges first) that each touch two
+ * rows of U [n_users, k], V [n_items, k] and Z: SoRec's edge (i, j) updates U[i] and Z[j] (Z is [n_users, k]) with the
+ * step lambda_c * learning_rate rounded to f32, MCF's updates V[i] and Z[j] (Z is [n_items, k]) with learning_rate; a
+ * rating (u, i) updates U[u] and V[i].  With the three matrices in one row space, the level rule of b200_pmf_schedule
+ * applies unchanged to the mixed stream.
+ *
+ * b200_cofactor_schedule (HOST): net_a, net_b host int32[n_edges] (user ids for SoRec, item ids for MCF), uid, iid host
+ * int32[n_ratings], all in stored order.
+ *   order       host int32[n_edges + n_ratings]: the stored index of each slot (edges [0, n_edges), rating r at
+ *               n_edges + r), level-major, stored order inside a level
+ *   level_ptr   host int32[n_edges + n_ratings + 1] (capacity); n_levels host int32
+ *
+ * b200_cofactor_fit: n_epochs epochs in one launch (one CTA walking the levels, a barrier between consecutive levels).
+ *   a_id, b_id, val device int32 / int32 / f32 [n_edges + n_ratings] in schedule order: the two row ids (within their
+ *                   matrices) and the target of each slot
+ *   is_edge         device uint8 [n_edges + n_ratings]: 1 for an edge slot, 0 for a rating slot
+ *   U, V, Z         device f64, updated in place; cache_u/v/z the RMSProp caches, same shapes (zero at the start of a
+ *                   fit, kept across calls).  A cache belongs to its matrix: both passes step SoRec's cache_u, MCF's cache_v
+ *   lambda_c        f32, SoRec only (ignored for MCF); lambda_reg (MCF's lamda), learning_rate, gamma f32
+ *   loss            device f64 [n_epochs, n_edges + n_ratings] or NULL: each update's loss term at its stored index;
+ *                   summing a row in stored order gives the reference's loss[epoch]
+ *   order           device int32[n_edges + n_ratings]; read only when loss != NULL
+ * Calling it twice with n_epochs = a and b is the same as calling it once with a + b.                                  */
+#define B200_COFACTOR_SOREC 0
+#define B200_COFACTOR_MCF 1
+B200_API int b200_cofactor_schedule(int variant, const int32_t* net_a, const int32_t* net_b, int64_t n_edges,
+                                    const int32_t* uid, const int32_t* iid, int64_t n_ratings, int64_t n_users,
+                                    int64_t n_items, int32_t* order, int32_t* level_ptr, int32_t* n_levels);
+B200_API int b200_cofactor_fit(int variant, const int32_t* a_id, const int32_t* b_id, const float* val,
+                               const uint8_t* is_edge, const int32_t* level_ptr, int32_t n_levels, int64_t n_edges,
+                               int64_t n_ratings, int k, double* U, double* V, double* Z, double* cache_u, double* cache_v,
+                               double* cache_z, int n_epochs, float lambda_c, float lambda_reg, float learning_rate,
+                               float gamma, double* loss, const int32_t* order, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * NMF (cornac/models/nmf/recom_nmf.pyx:182-267), multiplicative updates in plain IEEE f32, bit-identical to the
  * reference's serial loop.  Per epoch: a pass over the ratings in stored (CSR) order computes each prediction rp and,
  * with use_bias, steps the biases; then U and V are updated element-wise from ordered sums over each user's row and each
