@@ -852,7 +852,18 @@ struct DetState {
     DetPlan plan[2];                // by round parity
     unsigned long long* acc;        // [cap][k + 1] 2^-40 fixed-point sums of the shared rows; column k = the item bias
     unsigned int* n_shared;         // [rounds] slots taken by each round
+    float d_max;                    // bound on |d| that keeps every round sum in range (det_delta_bound)
 };
+
+// Largest |d| a delta may have in rounds of R samples: 2^(22 - ceil(log2 R)), 256 at R = 16384.  A live sample touches
+// each row at most once (one user row; i != j), so an element takes at most R terms per round and |Q| <= 2^62: the
+// int64 sum cannot wrap into a finite, wrong value.
+static float det_delta_bound(int64_t R)
+{
+    int c = 0;
+    while (((int64_t)1 << c) < R) ++c;
+    return ldexpf(1.f, 22 - c);
+}
 
 // x + d as the global f32 atomic add computes it (round to nearest, subnormal inputs and results flushed to zero)
 __device__ __forceinline__ float det_fadd(float x, float d)
@@ -869,11 +880,11 @@ struct DetDst {
     unsigned long long* a;
 };
 
-// An update that is not finite or beyond the fixed-point range (|d| >= 2^22) cannot be summed: the element it belongs to
-// becomes NaN at once, so a diverging model shows NaN as under the Hogwild kernels instead of saturated sums.
-__device__ __forceinline__ void det_put(const DetDst& t, int e, float d, float x)
+// An update that is not finite or not below the round's bound d_max cannot be summed: the element it belongs to becomes
+// NaN at once, so a diverging model shows NaN as under the Hogwild kernels instead of wrapped sums.
+__device__ __forceinline__ void det_put(const DetDst& t, int e, float d, float x, float d_max)
 {
-    if (!(fabsf(d) < 4194304.f)) {
+    if (!(fabsf(d) < d_max)) {
         __stcg(t.x + e, __int_as_float(0x7fc00000));
         return;
     }
@@ -1026,18 +1037,19 @@ __global__ void __launch_bounds__(256, 4) bpr_det_grad_kernel(const BprParams p,
             float z;
             if (sample_z(p.hinge, p.exact_exp, score, z, n_correct)) {
                 const float lr = p.lr, reg = p.reg;
+                const float d_max = d.d_max;
                 auto step = [&](int e, float uf, float vi, float vj) {
-                    det_put(du, e, lr * (z * (vi - vj) - reg * uf), uf);
-                    det_put(di, e, lr * (z * uf - reg * vi), vi);
-                    det_put(dj, e, lr * (-z * uf - reg * vj), vj);
+                    det_put(du, e, lr * (z * (vi - vj) - reg * uf), uf, d_max);
+                    det_put(di, e, lr * (z * uf - reg * vi), vi, d_max);
+                    det_put(dj, e, lr * (-z * uf - reg * vj), vj, d_max);
                 };
 #pragma unroll
                 for (int x = 0; x < DET_RC; ++x)
                     if (lane + 32 * x < k) step(lane + 32 * x, ru[x], ri[x], rj[x]);
                 for (int e = lane + 32 * DET_RC; e < k; e += 32) step(e, __ldcg(pu + e), __ldcg(pi + e), __ldcg(pj + e));
                 if (p.use_bias && lane == 0) {
-                    det_put(DetDst{p.B + i, di.a ? di.a + k : nullptr}, 0, lr * (z - reg * bi), bi);
-                    det_put(DetDst{p.B + j, dj.a ? dj.a + k : nullptr}, 0, lr * (-z - reg * bj), bj);
+                    det_put(DetDst{p.B + i, di.a ? di.a + k : nullptr}, 0, lr * (z - reg * bi), bi, d_max);
+                    det_put(DetDst{p.B + j, dj.a ? dj.a + k : nullptr}, 0, lr * (-z - reg * bj), bj, d_max);
                 }
             }
             // a row touched once is reset by its only toucher, after every lane has read its count
@@ -1110,6 +1122,7 @@ static int bpr_epoch_deterministic(const BprParams& p, int64_t n_users, cudaStre
     char* buf = nullptr;
     B200_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), bytes, st));
     DetState d;
+    d.d_max = det_delta_bound(round);
     d.acc = reinterpret_cast<unsigned long long*>(buf + rec_b);
     d.n_shared = reinterpret_cast<unsigned int*>(buf + rec_b + acc_b);
     unsigned int* cnt = d.n_shared + n_rounds;
