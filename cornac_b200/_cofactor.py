@@ -1,4 +1,4 @@
-"""The fit and device scoring shared by the SoRec and MCF plug-ins (recom_sorec.py, recom_mcf.py).
+"""The fit and rank() shared by the SoRec and MCF plug-ins (recom_sorec.py, recom_mcf.py).
 
 Both reference loops (cornac/models/sorec/cython/sorec.pyx, cornac/models/mcf/cython/mcf.pyx) draw U, V and Z from one
 generator and then run, per epoch, PMF's non-linear RMSProp update over the graph edges and then over the ratings.  The
@@ -71,28 +71,12 @@ class CofactorMixin:
         for x, d in zip((U, V, Z), dev):
             x[...] = d.cpu().numpy()
         self.U, self.V, self.Z = U, V, Z
-        exact = U.shape == (self.num_users, self.k) and V.shape == (self.num_items, self.k)
-        self._b200_dev = dict(U=dev[0], V=dev[1]) if exact else None
+        if U.shape == (self.num_users, self.k) and V.shape == (self.num_items, self.k):
+            self._b200_dev = dict(U=dev[0], V=dev[1])           # the trained device factors score as they are
 
-    # ---- device scores ---------------------------------------------------------------------------------------------
     def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
         """Recommender.rank (cornac/models/recommender.py:475-530) as written, over the f64 score row of score(u): the head
         of k items sorted and the rest in argpartition's order, or the whole argsort reversed for k == -1.  The examples of
         both models score NDCG over the whole list (NDCG(k=-1)) beside top-20 metrics, so the order of the tail is part of
-        the metric; F64RankingMixin.rank would order it by item id.  rank_batch / recommend_batch keep the mixin's order."""
+        the metric; ScoringMixin.rank would order it by item id.  rank_batch / recommend_batch keep the shared order."""
         return Recommender.rank(self, user_idx, item_indices, k, **kwargs)
-
-    def _b200_device(self):
-        if getattr(self, "_b200_dev", None) is None:          # None after fit(); absent after load()
-            engine.require_cuda()
-            self._b200_dev = dict(U=engine.to_device(np.ascontiguousarray(self.U[: self.num_users]), torch.float64),
-                                  V=engine.to_device(np.ascontiguousarray(self.V[: self.num_items]), torch.float64))
-        return self._b200_dev
-
-    def _scores_dev(self, user_indices):
-        """[n_q, num_items] f64 device scores V.dot(U[u]) of known users."""
-        d = self._b200_device()
-        user_indices = np.asarray(user_indices, dtype=np.int64)
-        if user_indices.size and (int(user_indices.min()) < 0 or int(user_indices.max()) >= self.num_users):
-            raise IndexError("user index out of bounds for the %d users of the model" % self.num_users)
-        return engine.score_batch_f64(d["U"], d["V"], user_idx=engine.to_device(user_indices, torch.int64))

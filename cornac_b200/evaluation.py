@@ -75,7 +75,7 @@ def _supported(model, metrics, exclude_unknowns, train_set):
         else:
             return False
     try:
-        n_score = model._b200_device()["n_items"]
+        n_score = model._b200_shape()[1]
     except Exception:
         return False
     return n_score >= train_set.num_items                   # every train item has a score row
@@ -123,7 +123,7 @@ def ranking_eval(model, metrics, train_set, test_set, val_set=None, rating_thres
     full_test = _positives(test_set.csr_matrix, rating_threshold, n_rows, test_set.csr_matrix.shape[1])
     users = np.fromiter((u for u in set(test_set.uir_tuple[0]) if full_test.indptr[u + 1] > full_test.indptr[u]),
                         dtype=np.int64)
-    n_model_users = int(model._b200_device()["U"].shape[0])
+    n_model_users = model._b200_shape()[0]
     if len(users) and (users.max() >= n_model_users or users.min() < 0
                        or np.any(test_pos.indptr[users + 1] == test_pos.indptr[users])):
         # users the model has no row for (the reference scores them through its unknown-user branch), or whose test
@@ -170,7 +170,6 @@ def _full_vector_metrics(model, metrics, users, test_pos, excl, n_items, pos_ptr
         AUC = sum_p (less_p - lessP_p) / (|P| (|C| - |P|))                         ranking.py:473-485
         AP  = mean_p ((|P| - lessP_p) / (|C| - less_p))      rankdata(.., "max")   ranking.py:522-525
         MRR = 1 / (1 + #{c ranked ahead of the best positive})                     ranking.py:213-222"""
-    d = model._b200_device()
     n_users = len(users)
     batch = max(1, min(n_users, _SCORE_SLAB_BYTES // (4 * n_items)))
     less = torch.zeros(max(test_pos.nnz, 1), dtype=torch.int64, device="cuda")
@@ -180,10 +179,8 @@ def _full_vector_metrics(model, metrics, users, test_pos, excl, n_items, pos_ptr
     slab = torch.empty((batch, n_items), dtype=torch.float32, device="cuda")
     for b0 in range(0, n_users, batch):
         ub = users[b0:b0 + batch]
+        sc = model._scores_dev(ub, n_items=n_items, out=slab[: len(ub)])
         uidx = engine.to_device(ub, torch.int64)
-        uoff = None if d["user_off"] is None else d["user_off"][uidx].contiguous()
-        sc = engine.score_batch(d["U"], d["V"], user_idx=uidx, item_base=d["item_base"], user_off=uoff, n_items=n_items,
-                                out=slab[: len(ub)])
         ex = excl[ub]
         ex.sort_indices()
         ep = engine.to_device(ex.indptr.astype(np.int64), torch.int64)

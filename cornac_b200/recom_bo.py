@@ -113,13 +113,6 @@ class BaselineOnly(DeviceScoringMixin, Recommender):
         zv = np.zeros((self.num_items, 1), dtype=DTYPE)
         return zu, zv, item_base, np.asarray(self.u_biases, dtype=DTYPE), self.num_items
 
-    def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
-        hit = self._b200_cached_rank(user_idx, item_indices, k) if self.knows_user(user_idx) else None
-        if hit is not None:
-            return hit
-        known = torch.from_numpy(np.asarray(self.score(user_idx), dtype=DTYPE)).cuda()[None, :]
-        if known.shape[1] != self.total_items:               # unknown items get the MIN score (recommender.py:507-511)
-            allsc = torch.full((1, self.total_items), float(known.min().item()), dtype=torch.float32, device="cuda")
-            allsc[:, : self.num_items] = known
-            known = allsc
-        return self._b200_rank(known, item_indices, k)
+    # rank() orders the host score(u) row: the device row's __fadd_rn sums round differently from the host's f64 sum
+    def _b200_rank_row(self, user_idx):
+        return self.score(user_idx)

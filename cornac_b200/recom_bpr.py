@@ -13,15 +13,12 @@ Modes (chosen like the reference chooses its thread count, recom_bpr.pyx:132-137
 `mode` ("auto" | "replay" | "hogwild") overrides the choice; it is the only extra argument.
 """
 import numpy as np
-import torch
 
-from cornac.exception import ScoreException
 from cornac.models.recommender import ANNMixin, MEASURE_DOT, Recommender
 from cornac.utils import get_rng
 from cornac.utils.init_utils import uniform, zeros
 
 from . import engine
-from ._lib import B200Error
 from ._scoring import DeviceScoringMixin
 
 DTYPE = np.float32
@@ -149,19 +146,13 @@ class BPR(DeviceScoringMixin, Recommender, ANNMixin):
     # reference: recom_bpr.pyx:272-297
     def score(self, user_idx, item_idx=None):
         if item_idx is None:
-            cached = self._b200_cached_scores(user_idx)
-            return cached.copy() if cached is not None else self._b200_scores_dev([user_idx])[0].cpu().numpy()
+            return self._b200_row(user_idx)
         item_score = self.i_biases[item_idx]
         item_score += np.dot(self.u_factors[user_idx], self.i_factors[item_idx])
         return item_score
 
-    # reference: recommender.py:476-530
-    def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
-        hit = self._b200_cached_rank(user_idx, item_indices, k)          # filled by transform() before an evaluation
-        if hit is not None:
-            return hit
-        scores = self._b200_scores_dev([user_idx])          # [1, total_items]
-        return self._b200_rank(scores, item_indices, k)
+    def _b200_rank_row(self, user_idx):
+        return self._scores_dev([user_idx])[0]              # score(u) serves every factor row, known user or not
 
     def get_vector_measure(self):
         return MEASURE_DOT

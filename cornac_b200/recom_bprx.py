@@ -107,16 +107,11 @@ class VEBPR(DeviceScoringMixin, Recommender, ANNMixin):
     # reference: recom_vebpr.pyx:339-363
     def score(self, user_idx, item_idx=None):
         if item_idx is None:
-            cached = self._b200_cached_scores(user_idx)
-            return cached.copy() if cached is not None else self._b200_scores_dev([user_idx])[0].cpu().numpy()
+            return self._b200_row(user_idx)
         return np.dot(self.u_factor[user_idx], self.i_factor[item_idx])
 
-    # reference: recommender.py:476-530
-    def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
-        hit = self._b200_cached_rank(user_idx, item_indices, k)
-        if hit is not None:
-            return hit
-        return self._b200_rank(self._b200_scores_dev([user_idx]), item_indices, k)
+    def _b200_rank_row(self, user_idx):
+        return self._scores_dev([user_idx])[0]              # score(u) serves every factor row, known user or not
 
     def get_vector_measure(self):
         return MEASURE_DOT

@@ -12,10 +12,10 @@ from cornac.exception import ScoreException
 from cornac.models.recommender import ANNMixin, MEASURE_DOT, Recommender
 
 from . import engine
-from ._scoring import F64RankingMixin
+from ._scoring import ScoringMixin
 
 
-class EASE(F64RankingMixin, Recommender, ANNMixin):
+class EASE(ScoringMixin, Recommender, ANNMixin):
     """Embarrassingly Shallow Autoencoders for Sparse Data (Steck, WWW 2019), fitted on the GPU.
 
     Parameters are the reference's: name="EASEᴿ", lamb=500 (L2 regularisation added to the Gram matrix's diagonal),
@@ -32,13 +32,12 @@ class EASE(F64RankingMixin, Recommender, ANNMixin):
         self.seed = seed
         self.B = B
         self.U = U
-        self._b200_register_f64()
+        self._b200_register_ignored()
 
     # reference: recom_ease.py:57-97
     def fit(self, train_set, val_set=None):
         Recommender.fit(self, train_set, val_set)
-        self._b200_dev = None
-        self._b200_eval_cache = None
+        self._b200_invalidate()
         self.U = train_set.matrix
         B = engine.ease_fit(self.U, self.lamb, self.posB)
         self.B = B.cpu().numpy()
@@ -56,10 +55,7 @@ class EASE(F64RankingMixin, Recommender, ANNMixin):
     def _scores_dev(self, user_indices):
         """[n_q, num_items] f64 device scores X[u, :] . B of known users."""
         d = self._b200_device()
-        user_indices = np.asarray(user_indices, dtype=np.int64)
-        if user_indices.size and (int(user_indices.min()) < 0 or int(user_indices.max()) >= d["X"].n_rows):
-            raise IndexError("user index out of bounds for the %d users of the model" % d["X"].n_rows)
-        return engine.ease_score(d["B"], user_indices, d["X"])
+        return engine.ease_score(d["B"], self._b200_check_users(user_indices, d["X"].n_rows), d["X"])
 
     # reference: recom_ease.py:99-126
     def score(self, user_idx, item_idx=None):

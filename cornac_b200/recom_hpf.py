@@ -18,12 +18,12 @@ from cornac.utils import get_rng
 from cornac.utils.init_utils import gamma
 
 from . import engine
-from ._scoring import F64RankingMixin
+from ._scoring import F64DotScoringMixin
 
 _STATE = (("G_s", "Gs"), ("G_r", "Gr"), ("L_s", "Ls"), ("L_r", "Lr"))
 
 
-class HPF(F64RankingMixin, Recommender, ANNMixin):
+class HPF(F64DotScoringMixin, Recommender, ANNMixin):
     """Hierarchical Poisson Factorization (Gopalan, Hofman and Blei, UAI 2015), trained on the GPU.
 
     Parameters are the reference's: k=5, max_iter=100, name="HPF", trainable=True, verbose=False, hierarchical=True
@@ -31,6 +31,8 @@ class HPF(F64RankingMixin, Recommender, ANNMixin):
     init_params=None (a dict of f64 arrays: "G_s", "G_r" of shape (n_users, k), "L_s", "L_r" of shape (n_items, k) to
     start from, and "Theta", "Beta" to score with when trainable=False).
     """
+
+    _B200_FACTORS = ("Theta", "Beta")
 
     def __init__(self, k=5, max_iter=100, name="HPF", trainable=True, verbose=False, hierarchical=True, seed=None,
                  init_params=None):
@@ -52,13 +54,12 @@ class HPF(F64RankingMixin, Recommender, ANNMixin):
         self.Gr = self.init_params.get("G_r", None)
         self.Ls = self.init_params.get("L_s", None)
         self.Lr = self.init_params.get("L_r", None)
-        self._b200_register_f64()
+        self._b200_register_ignored()
 
     # reference: recom_hpf.py:110-180
     def fit(self, train_set, val_set=None):
         Recommender.fit(self, train_set, val_set)
-        self._b200_dev = None
-        self._b200_eval_cache = None
+        self._b200_invalidate()
         if self.trainable:
             X = train_set.csc_matrix
             rid, cid, val = sp.find(X)
@@ -103,23 +104,6 @@ class HPF(F64RankingMixin, Recommender, ANNMixin):
         self.Theta = Gs / Gr
         self.Beta = Ls / Lr
         self.Gs, self.Gr, self.Ls, self.Lr = Gs, Gr, Ls, Lr
-
-    # ---- device scores ---------------------------------------------------------------------------------------------
-    def _b200_device(self):
-        if getattr(self, "_b200_dev", None) is None:          # None after fit(); absent after load()
-            engine.require_cuda()
-            self._b200_dev = dict(
-                Theta=engine.to_device(np.ascontiguousarray(self.Theta[: self.num_users], dtype=np.float64), torch.float64),
-                Beta=engine.to_device(np.ascontiguousarray(self.Beta[: self.num_items], dtype=np.float64), torch.float64))
-        return self._b200_dev
-
-    def _scores_dev(self, user_indices):
-        """[n_q, num_items] f64 device scores Beta.dot(Theta[u]) of known users."""
-        d = self._b200_device()
-        user_indices = np.asarray(user_indices, dtype=np.int64)
-        if user_indices.size and (int(user_indices.min()) < 0 or int(user_indices.max()) >= self.num_users):
-            raise IndexError("user index out of bounds for the %d users of the model" % self.num_users)
-        return engine.score_batch_f64(d["Theta"], d["Beta"], user_idx=engine.to_device(user_indices, torch.int64))
 
     # reference: recom_hpf.py:182-213
     def score(self, user_idx, item_idx=None):

@@ -16,6 +16,7 @@ from cornac.models.recommender import Recommender
 from cornac.utils import get_rng
 
 from . import engine
+from ._scoring import EvalCacheMixin
 
 EPS = 1e-8
 SIMILARITIES = ["cosine", "pearson"]
@@ -53,9 +54,8 @@ def _bm25_weight(ui):
     return (K1 + 1.0) / (K1 * length_norm[X.row] + X.data) * idf[X.col] + EPS
 
 
-class _KNNBase(Recommender):
-    _B200_IGNORED = ("_b200_dev", "_b200_eval_cache")
-    _B200_EVAL_CACHE_BYTES = 1 << 30            # host budget of the transform() cache (f64 score rows of the test users)
+class _KNNBase(EvalCacheMixin, Recommender):
+    _B200_EVAL_TOP = 0                          # rank() sorts every candidate: the transform() cache keeps rows only
     _USER_MODE = None
 
     def __init__(self, name, k, similarity, mean_centered, weighting, amplify, num_threads, trainable, verbose, seed):
@@ -79,11 +79,7 @@ class _KNNBase(Recommender):
             self.num_threads = num_threads
         else:
             self.num_threads = multiprocessing.cpu_count()
-        for a in self._B200_IGNORED:
-            if a not in self.ignored_attrs:
-                self.ignored_attrs.append(a)
-        self._b200_dev = None
-        self._b200_eval_cache = None
+        self._b200_register_ignored()
 
     def _weighted(self, weight_mat, train_set):
         if self.weighting == "idf":
@@ -101,11 +97,11 @@ class _KNNBase(Recommender):
 
     def fit(self, train_set, val_set=None):
         Recommender.fit(self, train_set, val_set)
+        self._b200_invalidate()
         weight_mat, ui, self.mean_arr = self._host_prepare(train_set)
         self._keep_ratings(ui)
         S, self.sim_mat = engine.knn_similarity(weight_mat, self.amplify)
         self._b200_dev = dict(S=S, ratings=engine.KnnRatings(self._score_ratings(), self.mean_arr))
-        self._b200_eval_cache = None
         return self
 
     def _b200_device(self):
@@ -117,41 +113,6 @@ class _KNNBase(Recommender):
     def _scores_dev(self, user_indices):
         d = self._b200_device()
         return engine.knn_score(self._USER_MODE, d["S"], np.asarray(user_indices, dtype=np.int64), d["ratings"], int(self.k))
-
-    # ---- Recommender.transform: the score rows of every test user, computed in batches -------------------------------
-    def transform(self, test_set):
-        """`Recommender.transform` hook (cornac/models/recommender.py:410-421), called once by BaseMethod.evaluate before
-        the per-user loops of rating_eval / ranking_eval: the f64 score rows of all users of `test_set` are computed in a
-        few kernel calls and kept in host memory (skipped when they do not fit the budget), so that score(), rate() and
-        rank() of those users are host work."""
-        self._b200_eval_cache = None
-        if self._B200_EVAL_CACHE_BYTES <= 0:
-            return
-        try:
-            users = np.unique(np.asarray(test_set.uir_tuple[0], dtype=np.int64))
-        except Exception:
-            return
-        users = users[(users >= 0) & (users < self.num_users)]
-        if len(users) == 0 or len(users) * self.num_items * 8 > self._B200_EVAL_CACHE_BYTES:
-            return
-        rows = np.empty((len(users), self.num_items), dtype=np.float64)
-        batch = max(1, (256 << 20) // (8 * self.num_items))
-        for b0 in range(0, len(users), batch):
-            ub = users[b0:b0 + batch]
-            rows[b0:b0 + len(ub)] = self._scores_dev(ub).cpu().numpy()
-        pos_of = np.full(self.num_users, -1, dtype=np.int64)
-        pos_of[users] = np.arange(len(users))
-        self._b200_eval_cache = dict(pos_of=pos_of, scores=rows)
-
-    def _row(self, user_idx):
-        c = getattr(self, "_b200_eval_cache", None)
-        if c is not None and 0 <= user_idx < len(c["pos_of"]) and c["pos_of"][user_idx] >= 0:
-            return c["scores"][c["pos_of"][user_idx]]
-        return self._scores_dev([user_idx])[0].cpu().numpy()
-
-    def _score(self, user_idx, item_idx):
-        row = self._row(user_idx)
-        return row.copy() if item_idx is None else row[item_idx]
 
     def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
         """`Recommender.rank` (cornac/models/recommender.py:476-530) with the total order (score desc, item id asc)."""
@@ -198,7 +159,7 @@ class UserKNN(_KNNBase):
             raise ScoreException("Can't make score prediction for (user_id=%d)" % user_idx)
         if item_idx is not None and not self.knows_item(item_idx):
             raise ScoreException("Can't make score prediction for (item_id=%d)" % item_idx)
-        return self._score(user_idx, item_idx)
+        return self._b200_row(user_idx, item_idx)
 
 
 class ItemKNN(_KNNBase):
@@ -232,4 +193,4 @@ class ItemKNN(_KNNBase):
             raise ScoreException("Can't make score prediction for user %d" % user_idx)
         if item_idx is not None and self.is_unknown_item(item_idx):
             raise ScoreException("Can't make score prediction for item %d" % item_idx)
-        return self._score(user_idx, item_idx)
+        return self._b200_row(user_idx, item_idx)

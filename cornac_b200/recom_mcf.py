@@ -15,10 +15,10 @@ from cornac.models.recommender import ANNMixin, MEASURE_DOT, Recommender
 from cornac.utils.common import scale, sigmoid
 
 from ._cofactor import CofactorMixin
-from ._scoring import F64RankingMixin
+from ._scoring import F64DotScoringMixin
 
 
-class MCF(CofactorMixin, F64RankingMixin, Recommender, ANNMixin):
+class MCF(CofactorMixin, F64DotScoringMixin, Recommender, ANNMixin):
     """Matrix co-factorisation (Park et al., WWW 2017), trained on the GPU.
 
     Parameters are the reference's: k=5, max_iter=100, learning_rate=0.001, gamma=0.9, lamda=0.001, name="MCF",
@@ -45,13 +45,12 @@ class MCF(CofactorMixin, F64RankingMixin, Recommender, ANNMixin):
         self.U = self.init_params.get("U", None)
         self.V = self.init_params.get("V", None)
         self.Z = self.init_params.get("Z", None)
-        self._b200_register_f64()
+        self._b200_register_ignored()
 
     # reference: recom_mcf.py:110-191
     def fit(self, train_set, val_set=None):
         Recommender.fit(self, train_set, val_set)
-        self._b200_dev = None
-        self._b200_eval_cache = None
+        self._b200_invalidate()
         if self.trainable:
             if getattr(train_set, "item_graph", None) is None:
                 raise ValueError("MCF requires a train set with an item_graph modality (cornac.data.GraphModality)")

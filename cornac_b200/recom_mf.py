@@ -125,30 +125,15 @@ class MF(DeviceScoringMixin, Recommender, ANNMixin):
         if item_idx is not None and self.is_unknown_item(item_idx):
             raise ScoreException("Can't make score prediction for item %d" % item_idx)
         if item_idx is None:
-            if self.knows_user(user_idx):
-                cached = self._b200_cached_scores(user_idx)
-                return cached.copy() if cached is not None else self._b200_scores_dev([user_idx])[0].cpu().numpy()
-            return self.global_mean + self.i_biases
+            return self._b200_row(user_idx) if self.knows_user(user_idx) else self.global_mean + self.i_biases
         item_score = self.global_mean + self.i_biases[item_idx]
         if self.knows_user(user_idx):
             item_score += self.u_biases[user_idx]
             item_score += self.u_factors[user_idx].dot(self.i_factors[item_idx])
         return item_score
 
-    # reference: recommender.py:476-530
-    def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
-        hit = self._b200_cached_rank(user_idx, item_indices, k) if self.knows_user(user_idx) else None
-        if hit is not None:
-            return hit
-        if not self.knows_user(user_idx):
-            known = torch.from_numpy(np.asarray(self.global_mean + self.i_biases, dtype=DTYPE)).cuda()[None, :]
-        else:
-            known = self._b200_scores_dev([user_idx])       # [1, num_items]
-        if known.shape[1] != self.total_items:               # unknown items get the MIN score (:507-511)
-            allsc = torch.full((1, self.total_items), float(known.min().item()), dtype=torch.float32, device="cuda")
-            allsc[:, : self.num_items] = known
-            known = allsc
-        return self._b200_rank(known, item_indices, k)
+    def _b200_rank_row(self, user_idx):
+        return self._scores_dev([user_idx])[0] if self.knows_user(user_idx) else self.global_mean + self.i_biases
 
     def get_vector_measure(self):
         return MEASURE_DOT

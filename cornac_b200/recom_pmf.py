@@ -17,12 +17,12 @@ from cornac.utils.common import scale, sigmoid
 from cornac.utils.init_utils import normal
 
 from . import engine
-from ._scoring import F64RankingMixin
+from ._scoring import F64DotScoringMixin
 
 VARIANTS = ("linear", "non_linear")
 
 
-class PMF(F64RankingMixin, Recommender, ANNMixin):
+class PMF(F64DotScoringMixin, Recommender, ANNMixin):
     """Probabilistic Matrix Factorization (Mnih and Salakhutdinov, NIPS 2008), trained on the GPU.
 
     Parameters are the reference's: k=5, max_iter=100, learning_rate=0.001, gamma=0.9, lambda_reg=0.001, name="PMF",
@@ -49,13 +49,12 @@ class PMF(F64RankingMixin, Recommender, ANNMixin):
         self.init_params = {} if init_params is None else init_params
         self.U = self.init_params.get("U", None)
         self.V = self.init_params.get("V", None)
-        self._b200_register_f64()
+        self._b200_register_ignored()
 
     # reference: recom_pmf.py:108-189
     def fit(self, train_set, val_set=None):
         Recommender.fit(self, train_set)
-        self._b200_dev = None
-        self._b200_eval_cache = None
+        self._b200_invalidate()
         if self.trainable:
             uid, iid, rat = train_set.uir_tuple
             rat = np.array(rat, dtype="float32")
@@ -119,23 +118,8 @@ class PMF(F64RankingMixin, Recommender, ANNMixin):
         U[...] = Ud.cpu().numpy()
         V[...] = Vd.cpu().numpy()
         self.U, self.V = U, V
-        self._b200_dev = dict(U=Ud, V=Vd) if U.shape == (self.num_users, self.k) and V.shape == (self.num_items, self.k) else None
-
-    # ---- device scores ---------------------------------------------------------------------------------------------
-    def _b200_device(self):
-        if getattr(self, "_b200_dev", None) is None:          # None after fit(); absent after load()
-            engine.require_cuda()
-            self._b200_dev = dict(U=engine.to_device(np.ascontiguousarray(self.U[: self.num_users]), torch.float64),
-                                  V=engine.to_device(np.ascontiguousarray(self.V[: self.num_items]), torch.float64))
-        return self._b200_dev
-
-    def _scores_dev(self, user_indices):
-        """[n_q, num_items] f64 device scores V.dot(U[u]) of known users."""
-        d = self._b200_device()
-        user_indices = np.asarray(user_indices, dtype=np.int64)
-        if user_indices.size and (int(user_indices.min()) < 0 or int(user_indices.max()) >= self.num_users):
-            raise IndexError("user index out of bounds for the %d users of the model" % self.num_users)
-        return engine.score_batch_f64(d["U"], d["V"], user_idx=engine.to_device(user_indices, torch.int64))
+        if U.shape == (self.num_users, self.k) and V.shape == (self.num_items, self.k):
+            self._b200_dev = dict(U=Ud, V=Vd)                   # the trained device factors score as they are
 
     # reference: recom_pmf.py:191-222
     def score(self, user_idx, item_idx=None):

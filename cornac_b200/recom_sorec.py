@@ -15,7 +15,7 @@ from cornac.models.recommender import ANNMixin, MEASURE_DOT, Recommender
 from cornac.utils.common import scale, sigmoid
 
 from ._cofactor import CofactorMixin
-from ._scoring import F64RankingMixin
+from ._scoring import F64DotScoringMixin
 
 
 def link_weights(net_uid, net_jid, net_val):
@@ -28,7 +28,7 @@ def link_weights(net_uid, net_jid, net_val):
     return np.sqrt(j_in / (j_in + u_out)) * np.asarray(net_val, dtype=np.float64)
 
 
-class SoRec(CofactorMixin, F64RankingMixin, Recommender, ANNMixin):
+class SoRec(CofactorMixin, F64DotScoringMixin, Recommender, ANNMixin):
     """Social recommendation using probabilistic matrix factorisation (Ma et al., CIKM 2008), trained on the GPU.
 
     Parameters are the reference's: name="SoRec", k=5, max_iter=100, learning_rate=0.001, lambda_c=10, lambda_reg=0.001,
@@ -61,13 +61,12 @@ class SoRec(CofactorMixin, F64RankingMixin, Recommender, ANNMixin):
             x = getattr(self, key)
             if x is not None and x.shape[1] != self.k:
                 raise ValueError("initial parameters %s dimension error" % key)
-        self._b200_register_f64()
+        self._b200_register_ignored()
 
     # reference: recom_sorec.py:127-218
     def fit(self, train_set, val_set=None):
         Recommender.fit(self, train_set, val_set)
-        self._b200_dev = None
-        self._b200_eval_cache = None
+        self._b200_invalidate()
         if self.trainable:
             if getattr(train_set, "user_graph", None) is None:
                 raise ValueError("SoRec requires a train set with a user_graph modality (cornac.data.GraphModality)")

@@ -91,25 +91,8 @@ class WMF(DeviceScoringMixin, Recommender, ANNMixin):
         if item_idx is not None and self.is_unknown_item(item_idx):
             raise ScoreException("Can't make score prediction for item %d" % item_idx)
         if item_idx is None:
-            cached = self._b200_cached_scores(user_idx)
-            return cached.copy() if cached is not None else self._b200_scores_dev([user_idx])[0].cpu().numpy()
+            return self._b200_row(user_idx)
         return self.V[item_idx, :].dot(self.U[user_idx, :])
-
-    # reference: recommender.py:476-530
-    def rank(self, user_idx, item_indices=None, k=-1, **kwargs):
-        import torch
-        hit = None if self.is_unknown_user(user_idx) else self._b200_cached_rank(user_idx, item_indices, k)
-        if hit is not None:
-            return hit
-        if self.is_unknown_user(user_idx):                        # score() raises -> every item gets default_score() (:499-503)
-            known = torch.full((1, self.total_items), float(self.default_score()), dtype=torch.float32, device="cuda")
-        else:
-            known = self._b200_scores_dev([user_idx])             # [1, num_items]
-        if known.shape[1] != self.total_items:                    # unknown items get the MIN score (:507-511)
-            allsc = torch.full((1, self.total_items), float(known.min().item()), dtype=torch.float32, device="cuda")
-            allsc[:, : self.num_items] = known
-            known = allsc
-        return self._b200_rank(known, item_indices, k)
 
     def get_vector_measure(self):
         return MEASURE_DOT
