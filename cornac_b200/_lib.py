@@ -19,6 +19,9 @@ _c = ctypes
 _vp, _i64, _i32, _u64, _u32, _f32, _int = (_c.c_void_p, _c.c_int64, _c.c_int32, _c.c_uint64, _c.c_uint32,
                                            _c.c_float, _c.c_int)
 
+# B200_C2PF_PARAMS of include/b200cornac.h: variant, sizes, k, the ratings, the graph, (at, bt), the state
+_C2PF = [_int, _i64, _i64, _i64, _int] + [_vp] * 8 + [_i64] + [_vp] * 5 + [_c.c_double] * 2 + [_vp] * 9
+
 # name -> (restype, argtypes); mirrors include/b200cornac.h one to one
 SIGNATURES = {
     "b200_last_error": (_c.c_char_p, []),
@@ -82,6 +85,9 @@ SIGNATURES = {
                                _vp, _vp, _vp, _vp, _vp]),
     "b200_hpf_fit": (_int, [_int, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                             _vp, _vp, _int, _vp, _vp]),
+    "b200_c2pf_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64, _int]),
+    "b200_c2pf_update": (_int, _C2PF + [_vp] * 11),
+    "b200_c2pf_fit": (_int, _C2PF + [_int, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),

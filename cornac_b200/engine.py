@@ -14,6 +14,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     nmf_prepare / nmf_fit          <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
     ease_fit / ease_score          <-> EASE.fit / EASE.score (cornac/models/ease/recom_ease.py:57-126)
     hpf_fit / hpf_update / hpf_expect <-> hpf_cpp / pf_cpp   (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275)
+    c2pf_fit / c2pf_update  <-> c2pf_cpp / tc2pf_cpp / rc2pf_cpp  (cornac/models/c2pf/cpp/cpp_c2pf.cpp)
 """
 import numpy as np
 import scipy.sparse as _sp
@@ -1103,6 +1104,108 @@ def hpf_expect(shape, rate, out=None):
         raise B200Error("out must have shape %s" % (tuple(shape.shape),))
     check(L.b200_hpf_expect(ptr(shape), ptr(rate), shape.numel(), ptr(out), current_stream()), "b200_hpf_expect")
     return out
+
+
+C2PF_VARIANTS = {"c2pf": 0, "tc2pf": 1, "rc2pf": 2}
+
+
+class C2pfGraph:
+    """Device copy of C2PF's context graph: a symmetric n_items x n_items CSC pattern (c_ptr int32[n_items + 1], c_row
+    int32[n_edges], rows ascending in each column), the position c_mir of each entry's mirror, and util f64[n_items], the
+    column sums of the graph's values.  `ratings` is the HpfData of the same items; the scratch is kept here."""
+
+    def __init__(self, ratings, c_ptr, c_row, c_mir, util):
+        require_cuda()
+        self.ratings = ratings
+        d = ratings.n_items
+        c_ptr, c_row, c_mir = (np.asarray(x, dtype=np.int64) for x in (c_ptr, c_row, c_mir))
+        self.n_edges = len(c_row)
+        if len(c_ptr) != d + 1 or c_ptr[0] != 0 or c_ptr[-1] != self.n_edges or np.any(np.diff(c_ptr) < 0):
+            raise B200Error("c_ptr is not the column pointer of a %d-column pattern with %d entries" % (d, self.n_edges))
+        c_col = np.repeat(np.arange(d), np.diff(c_ptr))
+        if len(c_mir) != self.n_edges or len(util) != d:
+            raise B200Error("c_mir must hold %d values and util %d" % (self.n_edges, d))
+        if self.n_edges and (c_row.min() < 0 or c_row.max() >= d or c_mir.min() < 0 or c_mir.max() >= self.n_edges or
+                             not np.array_equal(c_row[c_mir], c_col) or not np.array_equal(c_col[c_mir], c_row)):
+            raise B200Error("c_mir does not map every entry (r, i) to a stored (i, r)")
+        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
+        self.c_ptr = to_device(c_ptr.astype(np.int32), torch.int32)
+        self.c_row = to_device(pad(c_row.astype(np.int32)), torch.int32)
+        self.c_col = to_device(pad(c_col.astype(np.int32)), torch.int32)
+        self.c_mir = to_device(pad(c_mir.astype(np.int32)), torch.int32)
+        self.util = to_device(pad(np.asarray(util, dtype=np.float64)), torch.float64)
+        self._work = {}
+
+    def workspace(self, k):
+        if k not in self._work:
+            r = self.ratings
+            nbytes = _lib.load().b200_c2pf_workspace_bytes(r.n_users, r.n_items, r.nnz, self.n_edges, int(k))
+            if nbytes < 0:
+                raise B200Error("bad C2PF sizes")
+            self._work = {k: torch.empty(nbytes // 8, dtype=torch.float64, device="cuda")}
+        return self._work[k]
+
+
+def _c2pf_args(graph, variant, at, bt, state):
+    """The B200_C2PF_PARAMS of a call.  state = (Gs, Gr, Ls, Lr, L2s, L2r, L3s, L3r, T3r), f64 device tensors; None for the
+    matrices the variant does not have (tc2pf: L2s, L2r; rc2pf: Ls, Lr)."""
+    if variant not in C2PF_VARIANTS:
+        raise B200Error("variant must be one of %s, got %r" % (sorted(C2PF_VARIANTS), variant))
+    r = graph.ratings
+    Gs = state[0]
+    _dev(Gs, torch.float64, "Gs")
+    k = int(Gs.shape[1]) if Gs.dim() == 2 else 0
+    absent = {"c2pf": (), "tc2pf": ("L2s", "L2r"), "rc2pf": ("Ls", "Lr")}[variant]
+    names = ("Gs", "Gr", "Ls", "Lr", "L2s", "L2r")
+    for t, name, rows in zip(state[:6], names, (r.n_users, r.n_users) + (r.n_items,) * 4):
+        if name in absent:
+            continue
+        _dev(t, torch.float64, name)
+        if t.dim() != 2 or int(t.shape[0]) != rows or int(t.shape[1]) != k or k < 1:
+            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, max(k, 1), tuple(t.shape)))
+    for t, name, size in zip(state[6:], ("L3s", "L3r", "T3r"), (max(graph.n_edges, 1),) * 2 + (r.n_items,)):
+        _dev(t, torch.float64, name)
+        if t.numel() != size:
+            raise B200Error("%s must hold %d values, got %d" % (name, size, t.numel()))
+    ptrs = [None if name in absent else ptr(t) for t, name in zip(state[:6], names)] + [ptr(t) for t in state[6:]]
+    return k, [C2PF_VARIANTS[variant], *r.args(), k, *r.arrays(), graph.n_edges, ptr(graph.c_ptr), ptr(graph.c_row),
+               ptr(graph.c_col), ptr(graph.c_mir), ptr(graph.util), float(at), float(bt)] + ptrs
+
+
+def c2pf_fit(graph, variant, at, bt, state, n_iter):
+    """One call of c2pf_cpp / tc2pf_cpp / rc2pf_cpp (cpp_c2pf.cpp) with the kappa prior (at, bt): n_iter iterations over
+    `graph` (C2pfGraph), updating the device state (see _c2pf_args) in place.  Two calls of a and b iterations with the
+    same (at, bt) equal one call of a + b."""
+    L = require_cuda()
+    k, args = _c2pf_args(graph, variant, at, bt, state)
+    if int(n_iter) < 0:
+        raise B200Error("n_iter must be >= 0, got %d" % int(n_iter))
+    check(L.b200_c2pf_fit(*args, int(n_iter), ptr(graph.workspace(k)), current_stream()), "b200_c2pf_fit")
+
+
+def c2pf_update(graph, variant, at, bt, state, expectations, given=(None, None, None, None)):
+    """One iteration from the expectations (Lt, Lb, L2b, L3b, Lb2) (f64 device tensors, None where the variant has none),
+    which are replaced by those the iteration computes.  given = (Lt, Lb, L2b, L3b): tensors to take in place of the
+    expectations the iteration would compute (None: compute)."""
+    L = require_cuda()
+    k, args = _c2pf_args(graph, variant, at, bt, state)
+    r = graph.ratings
+    absent = {"c2pf": (), "tc2pf": (2,), "rc2pf": (1,)}[variant]
+    sizes = (r.n_users * k, r.n_items * k, r.n_items * k, max(graph.n_edges, 1), r.n_items * k)
+    for j, (t, size) in enumerate(zip(expectations, sizes)):
+        if j in absent:
+            continue
+        _dev(t, torch.float64, "expectation %d" % j)
+        if t.numel() != size:
+            raise B200Error("expectation %d must hold %d values, got %d" % (j, size, t.numel()))
+    for j, (t, size) in enumerate(zip(given, sizes)):
+        if t is not None:
+            _dev(t, torch.float64, "given expectation %d" % j)
+            if t.numel() != size:
+                raise B200Error("given expectation %d must hold %d values, got %d" % (j, size, t.numel()))
+    opt = lambda t: None if t is None else ptr(t)                     # noqa: E731
+    check(L.b200_c2pf_update(*args, *[None if j in absent else ptr(t) for j, t in enumerate(expectations)],
+                             *[opt(t) for t in given], ptr(graph.workspace(k)), current_stream()), "b200_c2pf_update")
 
 
 def rank_pack_items(V, item_base=None, n_items=None):

@@ -445,6 +445,38 @@ B200_API int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, in
                           double* Ls, double* Lr, double* Kr, double* Tr, int max_iter, double* work, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * C2PF (cornac/models/c2pf/cpp/cpp_c2pf.cpp): the variational fit of Collaborative Context Poisson Factorization in f64,
+ * in the reference's update order.  variant 0 is c2pf_cpp, 1 tc2pf_cpp (L2 is L: L2s, L2r, L2b are ignored), 2 rc2pf_cpp
+ * (no L: Ls, Lr, Lb are ignored).  Arithmetic and expectations as for HPF above.
+ *
+ * The ratings are HPF's arrays.  The context graph is a symmetric n_items x n_items pattern with n_edges stored entries:
+ *   c_ptr, c_row, c_col      device CSC int32[n_items + 1] / int32[n_edges] / int32[n_edges] (the column of each entry),
+ *                            rows ascending in each column
+ *   c_mir                    device int32[n_edges]: the position of (i, r) for the entry (r, i)
+ *   util                     device f64[n_items]: the column sums of the graph's values (read by variant 0 only)
+ * State (device f64, updated in place): Gs, Gr [n_users, k]; Ls, Lr, L2s, L2r [n_items, k]; L3s, L3r [n_edges] in CSC
+ * order; T3r [n_items] (ones for variants 1 and 2, which never write it).  (at, bt) is the kappa prior of the call.
+ * work: device scratch of b200_c2pf_workspace_bytes(n_users, n_items, nnz, n_edges, k) bytes.
+ *
+ * b200_c2pf_update: one iteration from the expectations Lt [n_users, k], Lb, L2b, Lb2 [n_items, k], L3b [n_edges], which
+ *   are replaced by those the iteration computes.  Each given_* that is not NULL is taken in place of the expectation the
+ *   iteration would compute at that point; with all four given the state is a fixed function of the inputs.
+ * b200_c2pf_fit: one call of the reference's fit: (variant 0) T3r from the state, the expectations, then n_iter
+ *   iterations, enqueued without a host synchronisation.  Two calls of a and b iterations with the same (at, bt) equal
+ *   one call of a + b.                                                                                                 */
+#define B200_C2PF_PARAMS                                                                                               \
+    int variant, int64_t n_users, int64_t n_items, int64_t nnz, int k, const int32_t *indptr, const int32_t *indices,  \
+        const int32_t *row, const double *val, const int32_t *csc_ptr, const int32_t *csc_row, const int32_t *csc_pos, \
+        const double *csc_val, int64_t n_edges, const int32_t *c_ptr, const int32_t *c_row, const int32_t *c_col,      \
+        const int32_t *c_mir, const double *util, double at, double bt, double *Gs, double *Gr, double *Ls, double *Lr, \
+        double *L2s, double *L2r, double *L3s, double *L3r, double *T3r
+B200_API int64_t b200_c2pf_workspace_bytes(int64_t n_users, int64_t n_items, int64_t nnz, int64_t n_edges, int k);
+B200_API int b200_c2pf_update(B200_C2PF_PARAMS, double* Lt, double* Lb, double* L2b, double* L3b, double* Lb2,
+                              const double* given_Lt, const double* given_Lb, const double* given_L2b,
+                              const double* given_L3b, double* work, void* stream);
+B200_API int b200_c2pf_fit(B200_C2PF_PARAMS, int n_iter, double* work, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
