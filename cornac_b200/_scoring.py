@@ -292,6 +292,22 @@ class DeviceScoringMixin(ScoringMixin):
         d = self._b200_device()
         return int(d["U"].shape[0]), d["n_items"]
 
+    def _b200_scores_nan_free(self):
+        """True when no score row can hold NaN.  score_batch sums U[u] . V[i] in f64, where products and sums of finite
+        f32 values cannot overflow, and rounds it to f32 once; so a NaN needs a non-finite parameter, or an f32 sum
+        item_base[i] + user_off[u] that overflows to inf next to a dot product that rounds to the opposite inf."""
+        d = self._b200_device()
+        bound = 0.0
+        for name in ("U", "V", "item_base", "user_off"):
+            t = d[name]
+            if t is None or t.numel() == 0:
+                continue
+            if not bool(torch.isfinite(t).all()):
+                return False
+            if name in ("item_base", "user_off"):
+                bound += float(t.abs().max())
+        return bound <= float(np.finfo(np.float32).max)
+
     def _b200_packed_items(self, n_rank):
         """fp16 tile images of the item side for the fused rank, built once per (trained model, candidate count) and kept
         with the device cache: V and the item base are constant until the next fit() / parameter change, which drops

@@ -180,10 +180,12 @@ rank_counts_kernel(const float* __restrict__ scores, long long n_q, long long n_
         const int bid = best_id;
         for (int p0 = 0; p0 < (npos > 0 ? npos : 1); p0 += FC_TILE) {
             const int np = min(FC_TILE, npos - p0);
-            // load + bitonic sort (ascending score) of this pass's positives; padding = +inf
+            // load + bitonic sort of this pass's positives, ascending by (float_key(score), position): a total order, also
+            // for +inf and NaN scores.  Padding = (the NaN of the largest key, INT_MAX) sorts after every positive, so the
+            // first np entries are exactly the pass's positives
             for (int t = tid; t < FC_TILE; t += FC_THREADS) {
-                sp[t] = t < np ? row[pos[p0 + t]] : INFINITY;
-                sidx[t] = t < np ? p0 + t : -1;
+                sp[t] = t < np ? row[pos[p0 + t]] : __int_as_float(0x7fffffff);
+                sidx[t] = t < np ? p0 + t : 0x7fffffff;
             }
             for (int t = tid; t <= FC_TILE; t += FC_THREADS) hist[t] = 0;
             __syncthreads();
@@ -196,9 +198,12 @@ rank_counts_kernel(const float* __restrict__ scores, long long n_q, long long n_
                         const int hi = lo + stride;
                         const bool asc = ((lo & size) == 0);
                         const float a = sp[lo], b = sp[hi];
-                        if ((a > b) == asc) {
+                        const int ia = sidx[lo], ib = sidx[hi];
+                        const unsigned long long ka = ((unsigned long long)::b200::float_key(a) << 32) | (unsigned)ia;
+                        const unsigned long long kb = ((unsigned long long)::b200::float_key(b) << 32) | (unsigned)ib;
+                        if ((ka > kb) == asc) {
                             sp[lo] = b; sp[hi] = a;
-                            const int ia = sidx[lo]; sidx[lo] = sidx[hi]; sidx[hi] = ia;
+                            sidx[lo] = ib; sidx[hi] = ia;
                         }
                     }
                     __syncthreads();

@@ -13,7 +13,8 @@ positives that are not test positives) and ALL users are handled in batches on t
     the reference's own formulas (ranking.py:473-485 AUC, :522-525 MAP, :213-222 MRR).
 
 Anything else (custom metrics, MRR next to @k metrics -- the reference then evaluates it on a partially sorted list --
-`exclude_unknowns=False`, models without the batched entry points) is delegated to the reference implementation unchanged.
+`exclude_unknowns=False`, models without the batched entry points, models whose scores could be NaN (a diverged fit), a
+test set without a positive at the threshold) is delegated to the reference implementation unchanged.
 Results are the numbers the reference loop produces with the same model (same order: score desc, item id asc).
 SURVEY.md section 8, row (f)2.
 """
@@ -78,7 +79,9 @@ def _supported(model, metrics, exclude_unknowns, train_set):
         n_score = model._b200_shape()[1]
     except Exception:
         return False
-    return n_score >= train_set.num_items                   # every train item has a score row
+    # every train item has a score row; and no score is NaN: b200_rank_counts reads NaN as an excluded item, while the
+    # reference loop keeps it as a candidate (a negative in AUC, a NaN MAP, a place in the ranked list)
+    return n_score >= train_set.num_items and model._b200_scores_nan_free()
 
 
 def _rank_within_segments(seg, score):
@@ -124,10 +127,11 @@ def ranking_eval(model, metrics, train_set, test_set, val_set=None, rating_thres
     users = np.fromiter((u for u in set(test_set.uir_tuple[0]) if full_test.indptr[u + 1] > full_test.indptr[u]),
                         dtype=np.int64)
     n_model_users = model._b200_shape()[0]
-    if len(users) and (users.max() >= n_model_users or users.min() < 0
-                       or np.any(test_pos.indptr[users + 1] == test_pos.indptr[users])):
-        # users the model has no row for (the reference scores them through its unknown-user branch), or whose test
-        # positives are all unknown items (the reference then divides by zero per metric): not batched
+    if (len(users) == 0 or users.max() >= n_model_users or users.min() < 0
+            or np.any(test_pos.indptr[users + 1] == test_pos.indptr[users])):
+        # no user with a test positive (the reference's average then divides by zero), users the model has no row for
+        # (the reference scores them through its unknown-user branch), or users whose test positives are all unknown
+        # items (the reference then divides by zero per metric): not batched, so the caller sees the reference's result
         return _reference_ranking_eval(model, metrics, train_set, test_set, val_set=val_set,
                                        rating_threshold=rating_threshold, exclude_unknowns=exclude_unknowns,
                                        verbose=verbose)
