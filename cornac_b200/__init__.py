@@ -9,7 +9,7 @@ Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b
 plug-ins).  The plug-in classes need the `cornac` package importable (they subclass its
 Recommender so that cornac.Experiment accepts them); the engine does not.
 """
-__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "HPF", "SoRec", "MCF", "C2PF", "engine", "B200Error"]
+__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "HPF", "SoRec", "MCF", "C2PF", "EFM", "engine", "B200Error"]
 
 from ._lib import B200Error  # noqa: F401
 
@@ -60,6 +60,9 @@ def __getattr__(name):
     if name == "C2PF":
         from .recom_c2pf import C2PF
         return C2PF
+    if name == "EFM":
+        from .recom_efm import EFM
+        return EFM
     if name == "BaselineOnly":
         from .recom_bo import BaselineOnly
         return BaselineOnly

@@ -21,6 +21,8 @@ _vp, _i64, _i32, _u64, _u32, _f32, _int = (_c.c_void_p, _c.c_int64, _c.c_int32, 
 
 # B200_C2PF_PARAMS of include/b200cornac.h: variant, sizes, k, the ratings, the graph, (at, bt), the state
 _C2PF = [_int, _i64, _i64, _i64, _int] + [_vp] * 8 + [_i64] + [_vp] * 5 + [_c.c_double] * 2 + [_vp] * 9
+# B200_EFM_DATA: per matrix (A, X, Y) ptr, row, idx, val, nnz, cptr, crow, cpos, cval; the two orders; the three sizes
+_EFM = ([_vp] * 4 + [_i64] + [_vp] * 4) * 3 + [_vp] * 2 + [_i64] * 3
 
 # name -> (restype, argtypes); mirrors include/b200cornac.h one to one
 SIGNATURES = {
@@ -88,6 +90,9 @@ SIGNATURES = {
     "b200_c2pf_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64, _int]),
     "b200_c2pf_update": (_int, _C2PF + [_vp] * 11),
     "b200_c2pf_fit": (_int, _C2PF + [_int, _vp, _vp]),
+    "b200_efm_csc": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp]),
+    "b200_efm_fit": (_int, _EFM + [_int, _int] + [_vp] * 7 + [_int] + [_f32] * 5 + [_vp, _vp]),
+    "b200_efm_queries": (_int, [_vp, _i64, _vp, _vp, _vp, _i64, _int, _int, _int, _c.c_double, _c.c_double, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),

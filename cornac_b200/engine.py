@@ -15,6 +15,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     ease_fit / ease_score          <-> EASE.fit / EASE.score (cornac/models/ease/recom_ease.py:57-126)
     hpf_fit / hpf_update / hpf_expect <-> hpf_cpp / pf_cpp   (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275)
     c2pf_fit / c2pf_update  <-> c2pf_cpp / tc2pf_cpp / rc2pf_cpp  (cornac/models/c2pf/cpp/cpp_c2pf.cpp)
+    efm_fit / efm_queries   <-> EFM._fit_efm / EFM.rank  (cornac/models/efm/recom_efm.pyx:268-353, 471-528)
 """
 import numpy as np
 import scipy.sparse as _sp
@@ -997,6 +998,119 @@ def nmf_fit(data, U, V, Bu, Bi, n_epochs, mu=0.0, learning_rate=0.005, lambda_u=
                          data.n_levels, k, ptr(U), ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs),
                          f32(mu), f32(learning_rate), f32(lambda_u), f32(lambda_v), f32(lambda_bu), f32(lambda_bi),
                          int(data.use_bias), ptr(loss), current_stream()), "b200_nmf_fit")
+
+
+def efm_csc(indptr, indices, n_cols):
+    """Host checks of a CSR and its stable CSC position map (b200_efm_csc, no device needed): (csc_ptr int32
+    [n_cols + 1], csc_pos int32 [nnz]); column c lists the stored indices of its entries in stored order."""
+    L = _lib.load()
+    indptr = np.ascontiguousarray(indptr, dtype=np.int32)
+    indices = np.ascontiguousarray(indices, dtype=np.int32)
+    csc_ptr = np.empty(int(n_cols) + 1, dtype=np.int32)
+    csc_pos = np.empty(len(indices), dtype=np.int32)
+    check(L.b200_efm_csc(ptr(indptr), ptr(indices), len(indptr) - 1, int(n_cols), len(indices), ptr(csc_ptr),
+                         ptr(csc_pos)), "b200_efm_csc")
+    return csc_ptr, csc_pos
+
+
+class EfmData:
+    """Device copy of EFM's three matrices, built once per fit and used by every iteration: for each of A (users x
+    items), X (users x aspects) and Y (items x aspects) the CSR with each entry's row and its stable CSC transpose
+    (b200_efm_csc); the launch orders of the item and aspect rows (longest chains first); the prediction buffer."""
+
+    def __init__(self, A, X, Y):
+        require_cuda()
+        A, X, Y = (_sp.csr_matrix(M) for M in (A, X, Y))
+        self.n_users, self.n_items = A.shape
+        self.n_aspects = X.shape[1]
+        if X.shape[0] != self.n_users or Y.shape != (self.n_items, self.n_aspects):
+            raise B200Error("A %s, X %s and Y %s do not agree in shape" % (A.shape, X.shape, Y.shape))
+        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
+        cols = {}
+        for name, M in (("a", A), ("x", X), ("y", Y)):
+            if M.nnz >= 2 ** 31:
+                raise B200Error("nnz >= 2^31 is not supported (int32 offsets)")
+            indptr = M.indptr.astype(np.int32)
+            indices = M.indices.astype(np.int32)
+            val = M.data.astype(np.float32)
+            row = np.repeat(np.arange(M.shape[0], dtype=np.int32), np.diff(indptr))
+            csc_ptr, csc_pos = efm_csc(indptr, indices, M.shape[1])
+            cols[name] = np.diff(csc_ptr)
+            setattr(self, "n" + name, int(M.nnz))
+            for field, a, dt in (("ptr", indptr, torch.int32), ("row", pad(row), torch.int32),
+                                 ("idx", pad(indices), torch.int32), ("val", pad(val), torch.float32),
+                                 ("cptr", csc_ptr, torch.int32), ("crow", pad(row[csc_pos]), torch.int32),
+                                 ("cpos", pad(csc_pos), torch.int32), ("cval", pad(val[csc_pos]), torch.float32)):
+                setattr(self, name + "_" + field, to_device(a, dt))
+        item_len = cols["a"] + np.diff(Y.indptr)
+        aspect_len = cols["x"] + cols["y"]
+        self.item_order = to_device(pad(np.argsort(-item_len, kind="stable").astype(np.int32)), torch.int32)
+        self.aspect_order = to_device(pad(np.argsort(-aspect_len, kind="stable").astype(np.int32)), torch.int32)
+        self.pred = torch.empty(max(self.na + self.nx + self.ny, 1), dtype=torch.float32, device="cuda")
+
+    def args(self):
+        """B200_EFM_DATA of include/b200cornac.h."""
+        out = []
+        for m in ("a", "x", "y"):
+            g = lambda f: getattr(self, m + "_" + f)                     # noqa: E731
+            out += [ptr(g("ptr")), ptr(g("row")), ptr(g("idx")), ptr(g("val")), getattr(self, "n" + m), ptr(g("cptr")),
+                    ptr(g("crow")), ptr(g("cpos")), ptr(g("cval"))]
+        return out + [ptr(self.item_order), ptr(self.aspect_order), self.n_users, self.n_items, self.n_aspects]
+
+
+def efm_fit(data, U1, U2, V, H1, H2, n_iter, lambda_x=1.0, lambda_y=1.0, lambda_u=0.01, lambda_h=0.01, lambda_v=0.01,
+            loss=None, workspace=None):
+    """n_iter iterations of EFM._fit_efm (recom_efm.pyx:268-353) over `data` (EfmData), updating the f32 device tensors
+    U1, U2, V, H1, H2 in place, bit for bit as the reference.s serial loop with the defined dot.
+    The hyperparameters are rounded to f32.  loss: optional f64 device tensor [n_iter] that receives each iteration's
+    loss, summed in f64 (not the reference's f32 order).  workspace: optional f32 device tensor of
+    efm_workspace_floats(...) floats (allocated per call otherwise)."""
+    L_ = require_cuda()
+    E = int(U1.shape[1]) if U1.dim() == 2 else 0
+    Lw = int(H1.shape[1]) if H1.dim() == 2 else 0
+    for t, name, shape in ((U1, "U1", (data.n_users, E)), (U2, "U2", (data.n_items, E)), (V, "V", (data.n_aspects, E)),
+                           (H1, "H1", (data.n_users, Lw)), (H2, "H2", (data.n_items, Lw))):
+        _dev(t, torch.float32, name)
+        if tuple(t.shape) != shape or E < 1 or Lw < 1:
+            raise B200Error("%s must have shape %s, got %s" % (name, shape, tuple(t.shape)))
+    if loss is not None:
+        _dev(loss, torch.float64, "loss")
+        if loss.numel() != int(n_iter):
+            raise B200Error("loss must hold n_iter = %d values" % int(n_iter))
+    need = efm_workspace_floats(data.n_users, data.n_items, data.n_aspects, E, Lw)
+    if workspace is None:
+        workspace = torch.empty(max(need, 1), dtype=torch.float32, device="cuda")
+    _dev(workspace, torch.float32, "workspace")
+    if workspace.numel() < need:
+        raise B200Error("workspace must hold %d floats" % need)
+    f32 = lambda x: float(np.float32(x))              # noqa: E731
+    check(L_.b200_efm_fit(*data.args(), E, Lw, ptr(U1), ptr(U2), ptr(V), ptr(H1), ptr(H2), ptr(workspace), ptr(data.pred),
+                          int(n_iter), f32(lambda_x), f32(lambda_y), f32(lambda_u), f32(lambda_h), f32(lambda_v),
+                          ptr(loss), current_stream()), "b200_efm_fit")
+
+
+def efm_workspace_floats(n_users, n_items, n_aspects, E, L):
+    """Floats of b200_efm_fit's workspace: the second buffer of each factor matrix."""
+    return (int(n_users) + int(n_items)) * (int(E) + int(L)) + int(n_aspects) * int(E)
+
+
+def efm_queries(U1, H1, V, num_most_cared, alpha, rating_scale, user_idx=None):
+    """[n_q, E + L] f32 query vectors of the aspect-weighted rank (b200_efm_queries) of the users user_idx (int64 device
+    tensor; None: every row of U1): Q[q] . [U2 | H2][i] is EFM.rank's row alpha * explicit + (1 - alpha) * score."""
+    L_ = require_cuda()
+    for t, name in ((U1, "U1"), (H1, "H1"), (V, "V")):
+        _dev(t, torch.float32, name)
+    E, Lw = int(U1.shape[1]), int(H1.shape[1])
+    if H1.shape[0] != U1.shape[0] or V.dim() != 2 or (V.shape[0] and int(V.shape[1]) != E):
+        raise B200Error("U1 %s, H1 %s and V %s do not agree in shape" % (tuple(U1.shape), tuple(H1.shape), tuple(V.shape)))
+    if user_idx is None:
+        user_idx = torch.arange(U1.shape[0], dtype=torch.int64, device=U1.device)
+    _dev(user_idx, torch.int64, "user_idx")
+    Q = torch.empty((user_idx.numel(), E + Lw), dtype=torch.float32, device=U1.device)
+    check(L_.b200_efm_queries(ptr(user_idx), user_idx.numel(), ptr(U1), ptr(H1), ptr(V), int(V.shape[0]), E, Lw,
+                              int(num_most_cared), float(alpha), float(rating_scale), ptr(Q), current_stream()),
+          "b200_efm_queries")
+    return Q
 
 
 class HpfData:

@@ -477,6 +477,51 @@ B200_API int b200_c2pf_update(B200_C2PF_PARAMS, double* Lt, double* Lb, double* 
 B200_API int b200_c2pf_fit(B200_C2PF_PARAMS, int n_iter, double* work, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * EFM (cornac/models/efm/recom_efm.pyx:268-353), multiplicative updates in plain IEEE f32 over the ratings A
+ * (n_users x n_items), the user aspect attentions X (n_users x n_aspects) and the item aspect qualities Y
+ * (n_items x n_aspects).  The predictions are the defined dot (f64 sum in index order of the exact f32 products, rounded
+ * once to f32; the A prediction f32(U1.U2) + f32(H1.H2)); everything else is the reference's f32 arithmetic and order,
+ * so the fit is bit-identical to oracle/efm_oracle.c.  Every accumulator reads the factors the iteration started with.
+ *
+ * b200_efm_csc (HOST): checks a CSR (indptr int32[n_rows + 1], indices int32[nnz] in [0, n_cols)) and builds its stable
+ *   CSC position map: csc_ptr int32[n_cols + 1], csc_pos int32[nnz] (the stored index of each CSC entry, stored order
+ *   inside a column).
+ *
+ * b200_efm_fit: n_iter iterations; two calls of a and b iterations equal one call of a + b.  B200_EFM_DATA, all device:
+ *   m_ptr, m_row, m_idx, m_val       the CSR of m = a, x, y (m_row: the row of each entry), nM entries
+ *   m_cptr, m_crow, m_cpos, m_cval   its CSC (b200_efm_csc): the row, stored index and value of each CSC entry
+ *   item_order    int32[n_items]: the order item rows are launched in (longest chains first)
+ *   aspect_order  int32[n_aspects]: the order aspect rows are launched in (longest chains first)
+ * U1 [n_users, E], U2 [n_items, E], V [n_aspects, E], H1 [n_users, L], H2 [n_items, L]: device f32, updated in place.
+ * work: device f32 workspace of (n_users + n_items) * (E + L) + n_aspects * E floats; pred: device f32 [nA + nX + nY]
+ * (the last iteration's predictions on return).  lambda_*: f32, as the reference's `floating` locals.  loss: device f64
+ * [n_iter] or NULL: += the reference's loss terms of each iteration, summed in f64 in no fixed order.
+ *
+ * b200_efm_queries: the query vector of each user users[q] (device int64[n_q]) for the aspect-weighted rank:
+ *   X_[a] = dot(U1[u], V[a]) (the defined dot); a_0..a_{m-1} the m = min(N, n_aspects) aspects of largest X_ (ties: the
+ *   smaller id first); with c = alpha / (N * rating_scale) and beta = 1 - alpha in f64,
+ *   Q[q, f] = f32(c * sum_t X_[a_t] V[a_t, f] + beta U1[u, f]) for f < E and Q[q, E + f] = f32(beta H1[u, f]) for f < L,
+ *   every f64 product and sum rounded separately, the sum over t ascending.  Q: device f32 [n_q, E + L].  Then
+ *   Q[q] . [U2 | H2][i] is, up to rounding, alpha * explicit(u, i) + (1 - alpha) * score(u, i): the row the reference's
+ *   rank() orders.                                                                                                      */
+#define B200_EFM_DATA                                                                                                   \
+    const int32_t *a_ptr, const int32_t *a_row, const int32_t *a_idx, const float *a_val, int64_t nA,                   \
+        const int32_t *a_cptr, const int32_t *a_crow, const int32_t *a_cpos, const float *a_cval, const int32_t *x_ptr,  \
+        const int32_t *x_row, const int32_t *x_idx, const float *x_val, int64_t nX, const int32_t *x_cptr,              \
+        const int32_t *x_crow, const int32_t *x_cpos, const float *x_cval, const int32_t *y_ptr, const int32_t *y_row,   \
+        const int32_t *y_idx, const float *y_val, int64_t nY, const int32_t *y_cptr, const int32_t *y_crow,             \
+        const int32_t *y_cpos, const float *y_cval, const int32_t *item_order, const int32_t *aspect_order,             \
+        int64_t n_users, int64_t n_items, int64_t n_aspects
+B200_API int b200_efm_csc(const int32_t* indptr, const int32_t* indices, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                          int32_t* csc_ptr, int32_t* csc_pos);
+B200_API int b200_efm_fit(B200_EFM_DATA, int E, int L, float* U1, float* U2, float* V, float* H1, float* H2, float* work,
+                          float* pred, int n_iter, float lambda_x, float lambda_y, float lambda_u, float lambda_h,
+                          float lambda_v, double* loss, void* stream);
+B200_API int b200_efm_queries(const int64_t* users, int64_t n_q, const float* U1, const float* H1, const float* V,
+                              int64_t n_aspects, int E, int L, int num_most_cared, double alpha, double rating_scale,
+                              float* Q, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Scores.  Replaces `out = base; fast_dot(U[u], V, out)` (fast_dot.pyx:40-43 as used by
  * BPR.score recom_bpr.pyx:290-293 and MF.score mf/recom_mf.py:272-278) for a BATCH of
  * query users:  out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]).
