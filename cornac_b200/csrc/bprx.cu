@@ -95,11 +95,14 @@ __global__ void __launch_bounds__(256) tri_hogwild_kernel(const TriParams p)
             }
         } else {
             // recom_sbpr.pyx:229-240: the entry at the sampled position is read -- and compared with j -- even for a user
-            // without social items (then it belongs to a later user; past the end of the array: nothing to compare)
+            // without social items (then it belongs to a later user; past the end of the array: nothing to compare).  The
+            // position can equal a_hi (fl(d3 * fl(1 / n_items)) rounds to 1 once n_items >= 2^24 - 1): the next user's
+            // entry and count, as the reference reads them, or -- for the last user -- no entry: the BPR fall-back.
             const int64_t kidx = (int64_t)a_lo + (int)floorf(((float)d3 * inv_items) * (float)n_aux_u);
-            const int32_t kid = kidx < p.n_aux ? __ldg(p.aux_items + kidx) : -1;
+            const bool in_array = kidx < p.n_aux;
+            const int32_t kid = in_array ? __ldg(p.aux_items + kidx) : -1;
             m.skip = m.skip || (m.j == kid);
-            if (n_aux_u > 0) { m.t = kid; m.t_count = __ldg(p.aux_counts + kidx); }
+            if (n_aux_u > 0 && in_array) { m.t = kid; m.t_count = __ldg(p.aux_counts + kidx); }
         }
         if (m.skip) { ++n_skipped; continue; }
 
@@ -314,20 +317,27 @@ __device__ __forceinline__ void tri_apply_exact(const TriParams& p, const TriSam
         const float s_uk = (float)(1.0 / (1.0 + (double)m.t_count));
         const float zik = sig_exact(__fmul_rn(score_ik, s_uk));
         const float zkj = sig_exact(score_kj);
+        // k can be i: a position at the end of the list reads the next user's entry, which may be one of u's own items.
+        // The reference then updates item_k / B[k] from the values item_i / B[i] have just been given.
+        const bool k_is_i = m.t == m.i;
         for (int f = lane; f < p.k; f += 32) {
-            const float u = __ldcg(pu + f), vi = __ldcg(pi + f), vj = __ldcg(pj + f), vk = __ldcg(pt + f);
-            const float eu = __fsub_rn(__fadd_rn(__fmul_rn(__fmul_rn(zik, __fsub_rn(vi, vk)), s_uk), __fmul_rn(zkj, __fsub_rn(vk, vj))),
+            const float u = __ldcg(pu + f), vi = __ldcg(pi + f), vj = __ldcg(pj + f), vk0 = __ldcg(pt + f);
+            const float eu = __fsub_rn(__fadd_rn(__fmul_rn(__fmul_rn(zik, __fsub_rn(vi, vk0)), s_uk), __fmul_rn(zkj, __fsub_rn(vk0, vj))),
                                        __fmul_rn(p.reg_u, u));
             __stcg(pu + f, __fadd_rn(u, __fmul_rn(lr, eu)));
-            __stcg(pi + f, __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(__fmul_rn(zik, u), s_uk), __fmul_rn(p.reg_v, vi)))));
+            const float vi_new = __fadd_rn(vi, __fmul_rn(lr, __fsub_rn(__fmul_rn(__fmul_rn(zik, u), s_uk), __fmul_rn(p.reg_v, vi))));
+            __stcg(pi + f, vi_new);
             __stcg(pj + f, __fadd_rn(vj, __fmul_rn(lr, __fsub_rn(__fmul_rn(-zkj, u), __fmul_rn(p.reg_v, vj)))));
+            const float vk = k_is_i ? vi_new : vk0;
             const float ek = __fsub_rn(__fsub_rn(__fmul_rn(zkj, u), __fmul_rn(__fmul_rn(zik, u), s_uk)), __fmul_rn(p.reg_v, vk));
             __stcg(pt + f, __fadd_rn(vk, __fmul_rn(lr, ek)));
         }
         if (p.use_bias && lane == 0) {
-            __stcg(p.B + m.i, __fadd_rn(bi, __fmul_rn(lr, __fsub_rn(__fmul_rn(zik, s_uk), __fmul_rn(p.reg_b, bi)))));
+            const float bi_new = __fadd_rn(bi, __fmul_rn(lr, __fsub_rn(__fmul_rn(zik, s_uk), __fmul_rn(p.reg_b, bi))));
+            __stcg(p.B + m.i, bi_new);
             __stcg(p.B + m.j, __fadd_rn(bj, __fmul_rn(lr, __fsub_rn(-zkj, __fmul_rn(p.reg_b, bj)))));
-            __stcg(p.B + m.t, __fadd_rn(bk, __fmul_rn(lr, __fsub_rn(__fsub_rn(zkj, __fmul_rn(zik, s_uk)), __fmul_rn(p.reg_b, bk)))));
+            const float bk_cur = k_is_i ? bi_new : bk;
+            __stcg(p.B + m.t, __fadd_rn(bk_cur, __fmul_rn(lr, __fsub_rn(__fsub_rn(zkj, __fmul_rn(zik, s_uk)), __fmul_rn(p.reg_b, bk_cur)))));
         }
     }
 }
@@ -348,9 +358,10 @@ __device__ __forceinline__ TriSample tri_resolve_stream(const TriParams& p, int6
         if (m.t >= 0) m.skip = m.skip || row_contains(p.aux_items, __ldg(p.aux_indptr + m.u), __ldg(p.aux_indptr + m.u + 1), m.j);
     } else {
         const int64_t kidx = p.k_index[s];
-        const int32_t kid = (kidx >= 0 && kidx < p.n_aux) ? __ldg(p.aux_items + kidx) : -1;
+        const bool in_array = kidx >= 0 && kidx < p.n_aux;
+        const int32_t kid = in_array ? __ldg(p.aux_items + kidx) : -1;
         m.skip = m.skip || (m.j == kid);
-        if (__ldg(p.aux_indptr + m.u + 1) > __ldg(p.aux_indptr + m.u)) { m.t = kid; m.t_count = __ldg(p.aux_counts + kidx); }
+        if (__ldg(p.aux_indptr + m.u + 1) > __ldg(p.aux_indptr + m.u) && in_array) { m.t = kid; m.t_count = __ldg(p.aux_counts + kidx); }
     }
     return m;
 }

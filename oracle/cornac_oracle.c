@@ -373,6 +373,8 @@ ORA_API void ora_vebpr_replay(const int64_t *i_index, const int32_t *v_ids, cons
  * k_index = the sampled position in the user's social-item list (social_indptr[u] + floor(k_rand * n_social));
  * k_id = social_item_ids[k_index] is read even when the user has NO social item (:231-233) -- then it is some
  * other user's entry (or, past the end of the array, undefined in the reference: here -1 = never equal to j).
+ * A user WITH social items whose position is past the end (k_index == n_social_total, which the float position
+ * reaches for the last such user once num_items >= 2^24 - 1) has no third item either: the BPR branch, as the kernels.
  * Returns 1 when skipped (:238-240).                                                                  */
 static int ora_sbpr_one(const int32_t *indptr, const int32_t *indices, int64_t u, int32_t i_id, int32_t j_id,
                         int64_t k_index, int32_t n_social, const int32_t *social_item_ids,
@@ -382,7 +384,7 @@ static int ora_sbpr_one(const int32_t *indptr, const int32_t *indices, int64_t u
     int32_t k_id = (k_index >= 0 && k_index < n_social_total) ? social_item_ids[k_index] : -1;
     if (ora_has_non_zero(indptr, indices, u, j_id) || j_id == k_id) return 1;
     float *user = U + (size_t)u * k, *item_i = V + (size_t)i_id * k, *item_j = V + (size_t)j_id * k;
-    if (n_social == 0) {                                            /* :247-265: BPR, biases always trained */
+    if (n_social == 0 || k_id < 0) {                                /* :247-265: BPR, biases always trained */
         float score = B[i_id] - B[j_id];
         for (int f = 0; f < k; ++f) score = score + user[f] * (item_i[f] - item_j[f]);
         float z = 1.0 / (1.0 + exp(score));
