@@ -19,10 +19,12 @@ _c = ctypes
 _vp, _i64, _i32, _u64, _u32, _f32, _int = (_c.c_void_p, _c.c_int64, _c.c_int32, _c.c_uint64, _c.c_uint32,
                                            _c.c_float, _c.c_int)
 
-# B200_C2PF_PARAMS of include/b200cornac.h: variant, sizes, k, the ratings, the graph, (at, bt), the state
-_C2PF = [_int, _i64, _i64, _i64, _int] + [_vp] * 8 + [_i64] + [_vp] * 5 + [_c.c_double] * 2 + [_vp] * 9
-# B200_EFM_DATA: per matrix (A, X, Y) ptr, row, idx, val, nnz, cptr, crow, cpos, cval; the two orders; the three sizes
-_EFM = ([_vp] * 4 + [_i64] + [_vp] * 4) * 3 + [_vp] * 2 + [_i64] * 3
+# B200_SPARSE of include/b200cornac.h: ptr, idx, row, val, nnz, cptr, crow, cpos, cval
+_SPARSE = [_vp] * 4 + [_i64] + [_vp] * 4
+# B200_C2PF_PARAMS: variant, sizes, k, the ratings, the graph, (at, bt), the state
+_C2PF = [_int, _i64, _i64, _int] + _SPARSE + [_i64] + [_vp] * 5 + [_c.c_double] * 2 + [_vp] * 9
+# B200_EFM_DATA: the matrices A, X, Y; the two orders; the three sizes
+_EFM = _SPARSE * 3 + [_vp] * 2 + [_i64] * 3
 
 # name -> (restype, argtypes); mirrors include/b200cornac.h one to one
 SIGNATURES = {
@@ -72,9 +74,9 @@ SIGNATURES = {
     "b200_cofactor_schedule": (_int, [_int, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "b200_cofactor_fit": (_int, [_int, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _int,
                                  _f32, _f32, _f32, _f32, _vp, _vp, _vp]),
-    "b200_nmf_prepare": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp]),
-    "b200_nmf_fit": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _int,
-                            _vp, _vp, _vp, _vp, _vp, _vp, _int, _f32, _f32, _f32, _f32, _f32, _f32, _int, _vp, _vp]),
+    "b200_csc_map": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp]),
+    "b200_nmf_fit": (_int, [_i64, _i64] + _SPARSE + [_vp] * 6 + [_i32, _int] + [_vp] * 6 + [_int] + [_f32] * 6 +
+                     [_int, _vp, _vp]),
     "b200_ease_gram_workspace_bytes": (_i64, [_i64]),
     "b200_ease_gram": (_int, [_i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _c.c_double, _vp, _vp, _vp]),
     "b200_spd_inverse_workspace_bytes": (_i64, [_i64]),
@@ -83,14 +85,11 @@ SIGNATURES = {
     "b200_ease_score": (_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_hpf_workspace_bytes": (_i64, [_i64, _i64, _i64, _int]),
     "b200_hpf_expect": (_int, [_vp, _vp, _i64, _vp, _vp]),
-    "b200_hpf_update": (_int, [_int, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                               _vp, _vp, _vp, _vp, _vp]),
-    "b200_hpf_fit": (_int, [_int, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                            _vp, _vp, _int, _vp, _vp]),
+    "b200_hpf_update": (_int, [_int, _i64, _i64, _int] + _SPARSE + [_vp] * 10),
+    "b200_hpf_fit": (_int, [_int, _i64, _i64, _int] + _SPARSE + [_vp] * 6 + [_int, _vp, _vp]),
     "b200_c2pf_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64, _int]),
     "b200_c2pf_update": (_int, _C2PF + [_vp] * 11),
     "b200_c2pf_fit": (_int, _C2PF + [_int, _vp, _vp]),
-    "b200_efm_csc": (_int, [_vp, _vp, _i64, _i64, _i64, _vp, _vp]),
     "b200_efm_fit": (_int, _EFM + [_int, _int] + [_vp] * 7 + [_int] + [_f32] * 5 + [_vp, _vp]),
     "b200_efm_queries": (_int, [_vp, _i64, _vp, _vp, _vp, _i64, _int, _int, _int, _c.c_double, _c.c_double, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),

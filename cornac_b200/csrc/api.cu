@@ -1,8 +1,10 @@
-// Library plumbing: error text, device info, the multi-GPU delta kernels.
+// Library plumbing: error text, device info, the CSC map of a sparse matrix, the multi-GPU delta kernels.
 #include <stdarg.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
+#include <vector>
 
 #include "common.cuh"
 
@@ -75,7 +77,7 @@ __global__ void delta_apply_kernel(float4* __restrict__ x, float4* __restrict__ 
 using namespace b200;
 
 extern "C" const char* b200_last_error(void) { return g_err; }
-extern "C" int b200_abi_version(void) { return 2; }
+extern "C" int b200_abi_version(void) { return 3; }
 extern "C" int64_t b200_kernel_launches(void) { return (int64_t)g_launches.load(std::memory_order_relaxed); }
 
 extern "C" int b200_device_info(int* sms, int* cc_major, int* cc_minor)
@@ -87,6 +89,31 @@ extern "C" int b200_device_info(int* sms, int* cc_major, int* cc_minor)
     if (sms) *sms = prop.multiProcessorCount;
     if (cc_major) *cc_major = prop.major;
     if (cc_minor) *cc_minor = prop.minor;
+    return B200_OK;
+}
+
+extern "C" int b200_csc_map(const int32_t* indptr, const int32_t* indices, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                            int32_t* csc_ptr, int32_t* csc_pos)
+{
+    B200_REQUIRE(nnz >= 0 && nnz < (1ll << 31) && n_rows >= 0 && n_cols >= 0 && n_rows < (1ll << 31) &&
+                     n_cols < (1ll << 31),
+                 "b200_csc_map: bad sizes n_rows=%lld n_cols=%lld nnz=%lld", (long long)n_rows, (long long)n_cols,
+                 (long long)nnz);
+    B200_REQUIRE(indptr && csc_ptr && (nnz == 0 || (indices && csc_pos)), "b200_csc_map: null pointer argument");
+    B200_REQUIRE(indptr[0] == 0 && indptr[n_rows] == nnz, "b200_csc_map: indptr spans [%d, %d], expected [0, %lld]",
+                 indptr[0], indptr[n_rows], (long long)nnz);
+    for (int64_t r = 0; r < n_rows; ++r)
+        B200_REQUIRE(indptr[r] <= indptr[r + 1], "b200_csc_map: indptr decreases at row %lld", (long long)r);
+    std::fill(csc_ptr, csc_ptr + n_cols + 1, 0);
+    for (int64_t j = 0; j < nnz; ++j) {
+        const int32_t c = indices[j];
+        B200_REQUIRE(c >= 0 && c < n_cols, "b200_csc_map: entry %lld has column %d outside [0, %lld)", (long long)j, c,
+                     (long long)n_cols);
+        ++csc_ptr[c + 1];
+    }
+    for (int64_t c = 0; c < n_cols; ++c) csc_ptr[c + 1] += csc_ptr[c];
+    std::vector<int32_t> next(csc_ptr, csc_ptr + n_cols);       // counting sort: stable, rows ascending in a column
+    for (int64_t j = 0; j < nnz; ++j) csc_pos[next[indices[j]]++] = (int32_t)j;
     return B200_OK;
 }
 

@@ -239,12 +239,9 @@ __global__ void __launch_bounds__(HPF_THREADS) c2pf_context_kernel(int64_t d, in
 
 struct C2pfArgs {
     int variant;
-    int64_t n, d, nnz;
+    int64_t n, d;
     int k;
-    const int32_t *indptr, *indices, *row;
-    const double* val;
-    const int32_t *csc_ptr, *csc_row, *csc_pos;
-    const double* csc_val;
+    SparseArgs<double> r;
     int64_t ne;
     const int32_t *c_ptr, *c_row, *c_col, *c_mir;
     const double* util;
@@ -325,8 +322,8 @@ void c2pf_update(C2pfArgs a, const C2pfExp& e, const C2pfExp& g, const C2pfWork&
         if (has_l) C2PF_LAUNCH(c2pf_add_kernel, dk_, e.Lb, e.Lb2, dk_, w.E);
     };
     auto dk_and_lbu = [&](bool lbu) {
-        C2PF_LAUNCH(hpf_dk_kernel, a.nnz, a.row, a.indices, a.nnz, k, e.Lt, E, w.dk);
-        if (lbu) C2PF_LAUNCH(c2pf_lbu_kernel, dk_, a.csc_ptr, a.csc_row, a.csc_val, a.csc_pos, w.dk, a.d, k, e.Lt, w.Lbu);
+        C2PF_LAUNCH(hpf_dk_kernel, a.r.nnz, a.r.row, a.r.idx, a.r.nnz, k, e.Lt, E, w.dk);
+        if (lbu) C2PF_LAUNCH(c2pf_lbu_kernel, dk_, a.r.cptr, a.r.crow, a.r.cval, a.r.cpos, w.dk, a.d, k, e.Lt, w.Lbu);
     };
     // 1. kappa
     item_side();
@@ -346,7 +343,7 @@ void c2pf_update(C2pfArgs a, const C2pfExp& e, const C2pfExp& g, const C2pfWork&
     if (a.variant == 0) C2PF_LAUNCH(c2pf_edge_sum_kernel<true>, a.d, a.d, a.c_ptr, a.c_mir, w.kap, a.at, a.bt, a.T3r);
     // 3. the users
     dk_and_lbu(false);
-    C2PF_LAUNCH(hpf_pass_kernel<true>, nk, a.indptr, a.indices, a.val, nullptr, w.dk, a.n, k, e.Lt, E, C2PF_SHAPE, a.Gs);
+    C2PF_LAUNCH(hpf_pass_kernel<true>, nk, a.r.ptr, a.r.idx, a.r.val, nullptr, w.dk, a.n, k, e.Lt, E, C2PF_SHAPE, a.Gs);
     if (has_l)
         C2PF_LAUNCH(c2pf_gr_terms_kernel<true>, (a.ne + a.d) * k, a.d, a.ne, k, a.c_ptr, a.c_row, a.c_col, a.c_mir, a.Ls,
                     a.Lr, a.L2s, a.L2r, w.kap, w.T);
@@ -360,7 +357,7 @@ void c2pf_update(C2pfArgs a, const C2pfExp& e, const C2pfExp& g, const C2pfWork&
     // 4. the items
     if (has_l) {
         dk_and_lbu(tied);
-        C2PF_LAUNCH(hpf_pass_kernel<false>, dk_, a.csc_ptr, a.csc_row, a.csc_val, a.csc_pos, w.dk, a.d, k, e.Lb, e.Lt,
+        C2PF_LAUNCH(hpf_pass_kernel<false>, dk_, a.r.cptr, a.r.crow, a.r.cval, a.r.cpos, w.dk, a.d, k, e.Lb, e.Lt,
                     C2PF_SHAPE, a.Ls);
     }
     if (a.variant == 0) {
@@ -380,16 +377,13 @@ void c2pf_update(C2pfArgs a, const C2pfExp& e, const C2pfExp& g, const C2pfWork&
 int c2pf_check(const C2pfArgs& a, const void* work, const char* what)
 {
     B200_REQUIRE(a.variant >= 0 && a.variant <= 2, "%s: bad variant %d", what, a.variant);
-    B200_REQUIRE(a.k >= 1 && a.n >= 0 && a.d >= 0 && a.nnz >= 0 && a.ne >= 0 && a.nnz < (1ll << 31) &&
-                     a.ne < (1ll << 31) && a.n < (1ll << 31) && a.d < (1ll << 31),
-                 "%s: bad sizes k=%d n_users=%lld n_items=%lld nnz=%lld n_edges=%lld", what, a.k, (long long)a.n,
-                 (long long)a.d, (long long)a.nnz, (long long)a.ne);
+    if (int rc = sparse_check(a.r, a.n, a.d, what)) return rc;
+    B200_REQUIRE(a.k >= 1 && a.ne >= 0 && a.ne < (1ll << 31), "%s: bad sizes k=%d n_edges=%lld", what, a.k,
+                 (long long)a.ne);
     const bool has_l = a.variant != 2, has_l2 = a.variant != 1;
-    B200_REQUIRE(a.indptr && a.csc_ptr && a.c_ptr && work && (a.n == 0 || (a.Gs && a.Gr)) &&
+    B200_REQUIRE(a.c_ptr && work && (a.n == 0 || (a.Gs && a.Gr)) &&
                      (a.d == 0 || ((!has_l || (a.Ls && a.Lr)) && (!has_l2 || (a.L2s && a.L2r)) && a.T3r && a.util)),
                  "%s: null pointer argument", what);
-    B200_REQUIRE(a.nnz == 0 || (a.indices && a.row && a.val && a.csc_row && a.csc_pos && a.csc_val),
-                 "%s: null rating arrays", what);
     B200_REQUIRE(a.ne == 0 || (a.c_row && a.c_col && a.c_mir && a.L3s && a.L3r), "%s: null graph arrays", what);
     return B200_OK;
 }
@@ -405,8 +399,8 @@ extern "C" int64_t b200_c2pf_workspace_bytes(int64_t n_users, int64_t n_items, i
 }
 
 #define B200_C2PF_ARGS                                                                                                 \
-    C2pfArgs a{variant, n_users, n_items, nnz, k, indptr, indices, row, val, csc_ptr, csc_row, csc_pos, csc_val,       \
-               n_edges, c_ptr, c_row, c_col, c_mir, util, at, bt, Gs, Gr, Ls, Lr, L2s, L2r, L3s, L3r, T3r}
+    C2pfArgs a{variant, n_users, n_items, k, B200_SPARSE_VIEW(r_), n_edges, c_ptr, c_row, c_col, c_mir, util, at, bt,  \
+               Gs, Gr, Ls, Lr, L2s, L2r, L3s, L3r, T3r}
 
 extern "C" int b200_c2pf_update(B200_C2PF_PARAMS, double* Lt, double* Lb, double* L2b, double* L3b, double* Lb2,
                                 const double* given_Lt, const double* given_Lb, const double* given_L2b,
@@ -420,7 +414,7 @@ extern "C" int b200_c2pf_update(B200_C2PF_PARAMS, double* Lt, double* Lb, double
     const C2pfExp e{Lt, Lb, L2b, L3b, Lb2};
     const C2pfExp g{const_cast<double*>(given_Lt), const_cast<double*>(given_Lb), const_cast<double*>(given_L2b),
                     const_cast<double*>(given_L3b), nullptr};
-    c2pf_update(a, e, g, c2pf_carve(work, n_users, n_items, nnz, n_edges, k), (cudaStream_t)stream);
+    c2pf_update(a, e, g, c2pf_carve(work, n_users, n_items, r_nnz, n_edges, k), (cudaStream_t)stream);
     B200_CUDA(cudaGetLastError());
     return B200_OK;
 }
@@ -431,7 +425,7 @@ extern "C" int b200_c2pf_fit(B200_C2PF_PARAMS, int n_iter, double* work, void* s
     if (int rc = c2pf_check(a, work, "b200_c2pf_fit")) return rc;
     B200_REQUIRE(n_iter >= 0, "b200_c2pf_fit: bad n_iter=%d", n_iter);
     cudaStream_t st = (cudaStream_t)stream;
-    const C2pfWork w = c2pf_carve(work, n_users, n_items, nnz, n_edges, k);
+    const C2pfWork w = c2pf_carve(work, n_users, n_items, r_nnz, n_edges, k);
     const C2pfExp& e = w.own;
     const int64_t dk_ = n_items * k;
     // What a call of the reference does before its loop: (c2pf) T3_r from kappa, the expectations, the context sums.

@@ -32,6 +32,33 @@ int sm_count();   // cached multiProcessorCount of the current device
 void count_launch(int n = 1);   // one tick per kernel this library launches (b200_kernel_launches)
 
 // ---------------------------------------------------------------------------
+// One sparse matrix as B200_SPARSE passes it: the CSR with each entry's row, and its stable CSC transpose (b200_csc_map)
+// with the row, CSR index and value of each CSC entry.
+template <class T>
+struct SparseArgs {
+    const int32_t *ptr, *idx, *row;
+    const T* val;
+    int64_t nnz;
+    const int32_t *cptr, *crow, *cpos;
+    const T* cval;
+};
+
+#define B200_SPARSE_VIEW(p) {p##ptr, p##idx, p##row, p##val, p##nnz, p##cptr, p##crow, p##cpos, p##cval}
+
+// The sizes and pointers of an n_rows x n_cols SparseArgs: int32 offsets, and the entry arrays present when nnz > 0.
+template <class T>
+int sparse_check(const SparseArgs<T>& m, int64_t n_rows, int64_t n_cols, const char* what)
+{
+    B200_REQUIRE(m.nnz >= 0 && m.nnz < (1ll << 31) && n_rows >= 0 && n_rows < (1ll << 31) && n_cols >= 0 &&
+                     n_cols < (1ll << 31),
+                 "%s: bad sizes n_rows=%lld n_cols=%lld nnz=%lld", what, (long long)n_rows, (long long)n_cols,
+                 (long long)m.nnz);
+    B200_REQUIRE(m.ptr && m.cptr, "%s: null pointer argument", what);
+    B200_REQUIRE(m.nnz == 0 || (m.idx && m.row && m.val && m.crow && m.cpos && m.cval), "%s: null entry arrays", what);
+    return B200_OK;
+}
+
+// ---------------------------------------------------------------------------
 // Philox4x32-10 counter-based RNG (Salmon et al., SC'11).  Stateless: the
 // (u,i,j) triplet of sample s in epoch e is a pure function of (seed, e, s),
 // so any grid shape / shard layout draws the same stream.

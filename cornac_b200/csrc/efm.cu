@@ -23,8 +23,6 @@
 #include "common.cuh"
 
 #include <algorithm>
-#include <numeric>
-#include <vector>
 
 namespace b200 {
 
@@ -92,13 +90,7 @@ __device__ __forceinline__ void efm_chain(const EfmSeg& s, int64_t r, int f, flo
 }
 
 struct EfmPass {
-    // CSR of A (users x items), its CSC map, X (users x aspects), Y (items x aspects) and the CSC maps of X and Y
-    const int32_t *a_ptr, *a_idx, *a_cptr, *a_crow, *a_cpos;
-    const float *a_val, *a_cval;
-    const int32_t *x_ptr, *x_idx, *x_cptr, *x_crow, *x_cpos;
-    const float *x_val, *x_cval;
-    const int32_t *y_ptr, *y_idx, *y_cptr, *y_crow, *y_cpos;
-    const float *y_val, *y_cval;
+    SparseArgs<float> a, x, y;                   // A (users x items), X (users x aspects), Y (items x aspects)
     const int32_t *item_order, *aspect_order;
     const float *pA, *pX, *pY;
     int64_t n_users, n_items, n_aspects;
@@ -181,36 +173,36 @@ __global__ void __launch_bounds__(EFM_WARPS * 32, 4) efm_pass_kernel(
         if (w < nw_a) {                                          // V[a]: X column a, then Y column a
             const int64_t a = __ldg(P.aspect_order + w / cE);
             const int q = (int)(w % cE);
-            const EfmSeg sx{P.x_cptr, P.x_crow, P.x_cval, P.x_cpos, P.pX, U1, P.E, P.lx};
-            const EfmSeg sy{P.y_cptr, P.y_crow, P.y_cval, P.y_cpos, P.pY, U2, P.E, P.ly};
-            const int cnt = (__ldg(P.x_cptr + a + 1) - __ldg(P.x_cptr + a)) + (__ldg(P.y_cptr + a + 1) - __ldg(P.y_cptr + a));
+            const EfmSeg sx{P.x.cptr, P.x.crow, P.x.cval, P.x.cpos, P.pX, U1, P.E, P.lx};
+            const EfmSeg sy{P.y.cptr, P.y.crow, P.y.cval, P.y.cpos, P.pY, U2, P.E, P.ly};
+            const int cnt = (__ldg(P.x.cptr + a + 1) - __ldg(P.x.cptr + a)) + (__ldg(P.y.cptr + a + 1) - __ldg(P.y.cptr + a));
             efm_update(sx, &sy, a, q * 32, P.E, cnt, P.lv, V, Vo, lsum, want_loss);
         } else if (w < nw_a + nw_i) {                            // U2[i]: A column i, then Y row i; H2[i]: A column i
             const int64_t v = w - nw_a;
             const int64_t i = __ldg(P.item_order + v / cR);
             const int q = (int)(v % cR);
-            const int cA = __ldg(P.a_cptr + i + 1) - __ldg(P.a_cptr + i);
+            const int cA = __ldg(P.a.cptr + i + 1) - __ldg(P.a.cptr + i);
             if (q < cE) {
-                const EfmSeg sa{P.a_cptr, P.a_crow, P.a_cval, P.a_cpos, P.pA, U1, P.E, 1.0f};
-                const EfmSeg sy{P.y_ptr, P.y_idx, P.y_val, nullptr, P.pY, V, P.E, P.ly};
-                const int cnt = cA + (__ldg(P.y_ptr + i + 1) - __ldg(P.y_ptr + i));
+                const EfmSeg sa{P.a.cptr, P.a.crow, P.a.cval, P.a.cpos, P.pA, U1, P.E, 1.0f};
+                const EfmSeg sy{P.y.ptr, P.y.idx, P.y.val, nullptr, P.pY, V, P.E, P.ly};
+                const int cnt = cA + (__ldg(P.y.ptr + i + 1) - __ldg(P.y.ptr + i));
                 efm_update(sa, &sy, i, q * 32, P.E, cnt, P.lu, U2, U2o, lsum, want_loss);
             } else {
-                const EfmSeg sa{P.a_cptr, P.a_crow, P.a_cval, P.a_cpos, P.pA, H1, P.L, 1.0f};
+                const EfmSeg sa{P.a.cptr, P.a.crow, P.a.cval, P.a.cpos, P.pA, H1, P.L, 1.0f};
                 efm_update(sa, nullptr, i, (q - cE) * 32, P.L, cA, P.lh, H2, H2o, lsum, want_loss);
             }
         } else {                                                 // U1[u]: A row u, then X row u; H1[u]: A row u
             const int64_t v = w - nw_a - nw_i;
             const int64_t u = v / cR;
             const int q = (int)(v % cR);
-            const int cA = __ldg(P.a_ptr + u + 1) - __ldg(P.a_ptr + u);
+            const int cA = __ldg(P.a.ptr + u + 1) - __ldg(P.a.ptr + u);
             if (q < cE) {
-                const EfmSeg sa{P.a_ptr, P.a_idx, P.a_val, nullptr, P.pA, U2, P.E, 1.0f};
-                const EfmSeg sx{P.x_ptr, P.x_idx, P.x_val, nullptr, P.pX, V, P.E, P.lx};
-                const int cnt = cA + (__ldg(P.x_ptr + u + 1) - __ldg(P.x_ptr + u));
+                const EfmSeg sa{P.a.ptr, P.a.idx, P.a.val, nullptr, P.pA, U2, P.E, 1.0f};
+                const EfmSeg sx{P.x.ptr, P.x.idx, P.x.val, nullptr, P.pX, V, P.E, P.lx};
+                const int cnt = cA + (__ldg(P.x.ptr + u + 1) - __ldg(P.x.ptr + u));
                 efm_update(sa, &sx, u, q * 32, P.E, cnt, P.lu, U1, U1o, lsum, want_loss);
             } else {
-                const EfmSeg sa{P.a_ptr, P.a_idx, P.a_val, nullptr, P.pA, H2, P.L, 1.0f};
+                const EfmSeg sa{P.a.ptr, P.a.idx, P.a.val, nullptr, P.pA, H2, P.L, 1.0f};
                 efm_update(sa, nullptr, u, (q - cE) * 32, P.L, cA, P.lh, H1, H1o, lsum, want_loss);
             }
         }
@@ -291,45 +283,19 @@ __global__ void __launch_bounds__(EFM_QUERY_THREADS) efm_query_kernel(
 
 using namespace b200;
 
-extern "C" int b200_efm_csc(const int32_t* indptr, const int32_t* indices, int64_t n_rows, int64_t n_cols, int64_t nnz,
-                            int32_t* csc_ptr, int32_t* csc_pos)
-{
-    B200_REQUIRE(nnz >= 0 && nnz < (1ll << 31) && n_rows >= 0 && n_cols >= 0 && n_rows < (1ll << 31) && n_cols < (1ll << 31),
-                 "b200_efm_csc: bad sizes n_rows=%lld n_cols=%lld nnz=%lld", (long long)n_rows, (long long)n_cols,
-                 (long long)nnz);
-    B200_REQUIRE(indptr && csc_ptr && (nnz == 0 || (indices && csc_pos)), "b200_efm_csc: null pointer argument");
-    B200_REQUIRE(indptr[0] == 0 && indptr[n_rows] == nnz, "b200_efm_csc: indptr spans [%d, %d], expected [0, %lld]",
-                 indptr[0], indptr[n_rows], (long long)nnz);
-    for (int64_t r = 0; r < n_rows; ++r)
-        B200_REQUIRE(indptr[r] <= indptr[r + 1], "b200_efm_csc: indptr decreases at row %lld", (long long)r);
-    std::fill(csc_ptr, csc_ptr + n_cols + 1, 0);
-    for (int64_t j = 0; j < nnz; ++j) {
-        const int32_t c = indices[j];
-        B200_REQUIRE(c >= 0 && c < n_cols, "b200_efm_csc: entry %lld has column %d outside [0, %lld)", (long long)j, c,
-                     (long long)n_cols);
-        ++csc_ptr[c + 1];
-    }
-    for (int64_t c = 0; c < n_cols; ++c) csc_ptr[c + 1] += csc_ptr[c];
-    std::vector<int32_t> next(csc_ptr, csc_ptr + n_cols);       // counting sort: stable, rows ascending in a column
-    for (int64_t j = 0; j < nnz; ++j) csc_pos[next[indices[j]]++] = (int32_t)j;
-    return B200_OK;
-}
-
 extern "C" int b200_efm_fit(B200_EFM_DATA, int E, int L, float* U1, float* U2, float* V, float* H1, float* H2,
                             float* work, float* pred, int n_iter, float lambda_x, float lambda_y, float lambda_u,
                             float lambda_h, float lambda_v, double* loss, void* stream)
 {
-    B200_REQUIRE(E >= 1 && L >= 1 && n_iter >= 0 && n_users >= 0 && n_items >= 0 && n_aspects >= 0 && nA >= 0 &&
-                     nX >= 0 && nY >= 0 && nA < (1ll << 31) && nX < (1ll << 31) && nY < (1ll << 31),
-                 "b200_efm_fit: bad sizes E=%d L=%d n_iter=%d n_users=%lld n_items=%lld n_aspects=%lld", E, L, n_iter,
-                 (long long)n_users, (long long)n_items, (long long)n_aspects);
-    B200_REQUIRE(a_ptr && a_cptr && x_ptr && x_cptr && y_ptr && y_cptr && item_order && aspect_order && U1 && U2 && V &&
-                     H1 && H2 && work && pred,
+    const EfmPass P{B200_SPARSE_VIEW(a_), B200_SPARSE_VIEW(x_), B200_SPARSE_VIEW(y_), item_order, aspect_order,
+                    pred, pred + a_nnz, pred + a_nnz + x_nnz, n_users, n_items, n_aspects, E, L, lambda_x, lambda_y,
+                    lambda_u, lambda_h, lambda_v};
+    if (int rc = sparse_check(P.a, n_users, n_items, "b200_efm_fit")) return rc;
+    if (int rc = sparse_check(P.x, n_users, n_aspects, "b200_efm_fit")) return rc;
+    if (int rc = sparse_check(P.y, n_items, n_aspects, "b200_efm_fit")) return rc;
+    B200_REQUIRE(E >= 1 && L >= 1 && n_iter >= 0, "b200_efm_fit: bad sizes E=%d L=%d n_iter=%d", E, L, n_iter);
+    B200_REQUIRE(item_order && aspect_order && U1 && U2 && V && H1 && H2 && work && pred,
                  "b200_efm_fit: null pointer argument");
-    B200_REQUIRE((nA == 0 || (a_row && a_idx && a_val && a_crow && a_cpos && a_cval)) &&
-                     (nX == 0 || (x_row && x_idx && x_val && x_crow && x_cpos && x_cval)) &&
-                     (nY == 0 || (y_row && y_idx && y_val && y_crow && y_cpos && y_cval)),
-                 "b200_efm_fit: null entry arrays");
     if (n_iter == 0) return B200_OK;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t sz[5] = {(size_t)n_users * E, (size_t)n_items * E, (size_t)n_aspects * E, (size_t)n_users * L,
@@ -340,11 +306,7 @@ extern "C" int b200_efm_fit(B200_EFM_DATA, int E, int L, float* U1, float* U2, f
         nxt[m] = work;
         work += sz[m];
     }
-    float *pA = pred, *pX = pred + nA, *pY = pred + nA + nX;
-    const EfmPass P{a_ptr, a_idx, a_cptr, a_crow, a_cpos, a_val, a_cval, x_ptr, x_idx, x_cptr, x_crow, x_cpos, x_val,
-                    x_cval, y_ptr, y_idx, y_cptr, y_crow, y_cpos, y_val, y_cval, item_order, aspect_order, pA, pX, pY,
-                    n_users, n_items, n_aspects, E, L, lambda_x, lambda_y, lambda_u, lambda_h, lambda_v};
-    const int64_t n_pred = nA + nX + nY;
+    const int64_t n_pred = a_nnz + x_nnz + y_nnz;
     const unsigned cap = (unsigned)sm_count() * 16;
     const unsigned grid_p = (unsigned)std::max<int64_t>(1, std::min<int64_t>(cap, (n_pred + EFM_PRED_THREADS - 1) / EFM_PRED_THREADS));
     const int64_t cR = (E + 31) / 32 + (L + 31) / 32;
@@ -353,9 +315,10 @@ extern "C" int b200_efm_fit(B200_EFM_DATA, int E, int L, float* U1, float* U2, f
     for (int it = 0; it < n_iter; ++it) {
         double* le = loss ? loss + it : nullptr;
         if (n_pred > 0) {
-            efm_pred_kernel<<<grid_p, EFM_PRED_THREADS, 0, st>>>(a_row, a_idx, a_val, nA, x_row, x_idx, x_val, nX, y_row,
-                                                                 y_idx, y_val, nY, cur[0], cur[1], cur[2], cur[3], cur[4],
-                                                                 E, L, pA, pX, pY, le);
+            efm_pred_kernel<<<grid_p, EFM_PRED_THREADS, 0, st>>>(a_row, a_idx, a_val, a_nnz, x_row, x_idx, x_val, x_nnz,
+                                                                 y_row, y_idx, y_val, y_nnz, cur[0], cur[1], cur[2],
+                                                                 cur[3], cur[4], E, L, pred, pred + a_nnz,
+                                                                 pred + a_nnz + x_nnz, le);
             ::b200::count_launch();
         }
         if (n_work > 0) {

@@ -78,12 +78,9 @@ void hpf_rate(int64_t n_rows, int k, const double* S, double* R, double* Kr, con
 
 struct HpfArgs {
     int hierarchical;
-    int64_t n_users, n_items, nnz;
+    int64_t n_users, n_items;
     int k;
-    const int32_t *indptr, *indices, *row;
-    const double* val;
-    const int32_t *csc_ptr, *csc_row, *csc_pos;
-    const double* csc_val;
+    SparseArgs<double> r;
     double *Gs, *Gr, *Ls, *Lr, *Kr, *Tr;
 };
 
@@ -102,13 +99,13 @@ void hpf_update(const HpfArgs& a, const double* Lt, const double* Lb, const HpfW
     }
     hpf_colsum_kernel<<<gk, 32, 0, st>>>(w.qL, a.n_items, k, w.S);
     count_launch();
-    if (a.nnz > 0) {
-        hpf_dk_kernel<<<hpf_grid(a.nnz), HPF_THREADS, 0, st>>>(a.row, a.indices, a.nnz, k, Lt, Lb, w.dk);
+    if (a.r.nnz > 0) {
+        hpf_dk_kernel<<<hpf_grid(a.r.nnz), HPF_THREADS, 0, st>>>(a.r.row, a.r.idx, a.r.nnz, k, Lt, Lb, w.dk);
         count_launch();
     }
     if (a.n_users > 0) {
         hpf_pass_kernel<true><<<hpf_grid(a.n_users * k), HPF_THREADS, 0, st>>>(
-            a.indptr, a.indices, a.val, nullptr, w.dk, a.n_users, k, Lt, Lb, HPF_A, a.Gs);
+            a.r.ptr, a.r.idx, a.r.val, nullptr, w.dk, a.n_users, k, Lt, Lb, HPF_A, a.Gs);
         count_launch();
     }
     if (a.hierarchical)
@@ -119,7 +116,7 @@ void hpf_update(const HpfArgs& a, const double* Lt, const double* Lb, const HpfW
     count_launch();
     if (a.n_items > 0) {
         hpf_pass_kernel<false><<<hpf_grid(a.n_items * k), HPF_THREADS, 0, st>>>(
-            a.csc_ptr, a.csc_row, a.csc_val, a.csc_pos, w.dk, a.n_items, k, Lb, Lt, HPF_B, a.Ls);
+            a.r.cptr, a.r.crow, a.r.cval, a.r.cpos, w.dk, a.n_items, k, Lb, Lt, HPF_B, a.Ls);
         count_launch();
     }
     if (a.hierarchical)
@@ -130,15 +127,10 @@ void hpf_update(const HpfArgs& a, const double* Lt, const double* Lb, const HpfW
 
 int hpf_check(const HpfArgs& a, const void* work, const char* what)
 {
-    B200_REQUIRE(a.k >= 1 && a.n_users >= 0 && a.n_items >= 0 && a.nnz >= 0 && a.nnz < (1ll << 31) &&
-                     a.n_users < (1ll << 31) && a.n_items < (1ll << 31),
-                 "%s: bad sizes k=%d n_users=%lld n_items=%lld nnz=%lld", what, a.k, (long long)a.n_users,
-                 (long long)a.n_items, (long long)a.nnz);
-    B200_REQUIRE(a.indptr && a.csc_ptr && work && (a.n_users == 0 || (a.Gs && a.Gr && a.Kr)) &&
-                     (a.n_items == 0 || (a.Ls && a.Lr && a.Tr)),
+    if (int rc = sparse_check(a.r, a.n_users, a.n_items, what)) return rc;
+    B200_REQUIRE(a.k >= 1, "%s: bad k=%d", what, a.k);
+    B200_REQUIRE(work && (a.n_users == 0 || (a.Gs && a.Gr && a.Kr)) && (a.n_items == 0 || (a.Ls && a.Lr && a.Tr)),
                  "%s: null pointer argument", what);
-    B200_REQUIRE(a.nnz == 0 || (a.indices && a.row && a.val && a.csc_row && a.csc_pos && a.csc_val),
-                 "%s: null rating arrays", what);
     return B200_OK;
 }
 
@@ -161,35 +153,27 @@ extern "C" int b200_hpf_expect(const double* shape, const double* rate, int64_t 
     return B200_OK;
 }
 
-#define B200_HPF_ARGS                                                                                                  \
-    HpfArgs a{hierarchical, n_users, n_items, nnz, k, indptr, indices, row, val, csc_ptr, csc_row, csc_pos, csc_val,   \
-              Gs, Gr, Ls, Lr, Kr, Tr}
-
-extern "C" int b200_hpf_update(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k,
-                               const int32_t* indptr, const int32_t* indices, const int32_t* row, const double* val,
-                               const int32_t* csc_ptr, const int32_t* csc_row, const int32_t* csc_pos,
-                               const double* csc_val, const double* Lt, const double* Lb, double* Gs, double* Gr,
-                               double* Ls, double* Lr, double* Kr, double* Tr, double* work, void* stream)
+extern "C" int b200_hpf_update(int hierarchical, int64_t n_users, int64_t n_items, int k, B200_SPARSE(r_, double),
+                               const double* Lt, const double* Lb, double* Gs, double* Gr, double* Ls, double* Lr,
+                               double* Kr, double* Tr, double* work, void* stream)
 {
-    B200_HPF_ARGS;
+    const HpfArgs a{hierarchical, n_users, n_items, k, B200_SPARSE_VIEW(r_), Gs, Gr, Ls, Lr, Kr, Tr};
     if (int rc = hpf_check(a, work, "b200_hpf_update")) return rc;
     B200_REQUIRE((n_users == 0 || Lt) && (n_items == 0 || Lb), "b200_hpf_update: null Lt / Lb");
-    hpf_update(a, Lt, Lb, hpf_carve(work, n_users, n_items, nnz, k), (cudaStream_t)stream);
+    hpf_update(a, Lt, Lb, hpf_carve(work, n_users, n_items, r_nnz, k), (cudaStream_t)stream);
     B200_CUDA(cudaGetLastError());
     return B200_OK;
 }
 
-extern "C" int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k,
-                            const int32_t* indptr, const int32_t* indices, const int32_t* row, const double* val,
-                            const int32_t* csc_ptr, const int32_t* csc_row, const int32_t* csc_pos,
-                            const double* csc_val, double* Gs, double* Gr, double* Ls, double* Lr, double* Kr,
-                            double* Tr, int max_iter, double* work, void* stream)
+extern "C" int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, int k, B200_SPARSE(r_, double),
+                            double* Gs, double* Gr, double* Ls, double* Lr, double* Kr, double* Tr, int max_iter,
+                            double* work, void* stream)
 {
-    B200_HPF_ARGS;
+    const HpfArgs a{hierarchical, n_users, n_items, k, B200_SPARSE_VIEW(r_), Gs, Gr, Ls, Lr, Kr, Tr};
     if (int rc = hpf_check(a, work, "b200_hpf_fit")) return rc;
     B200_REQUIRE(max_iter >= 0, "b200_hpf_fit: bad max_iter=%d", max_iter);
     cudaStream_t st = (cudaStream_t)stream;
-    const HpfWork w = hpf_carve(work, n_users, n_items, nnz, k);
+    const HpfWork w = hpf_carve(work, n_users, n_items, r_nnz, k);
     // hpf_cpp's update_kappa_r before the loop.  After an iteration K_r and T_r already hold these values, so a fit split
     // into several calls recomputes them bit for bit.
     if (hierarchical) {
@@ -204,4 +188,3 @@ extern "C" int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, 
     B200_CUDA(cudaGetLastError());
     return B200_OK;
 }
-#undef B200_HPF_ARGS

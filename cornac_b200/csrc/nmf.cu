@@ -23,8 +23,6 @@
 #include "common.cuh"
 
 #include <algorithm>
-#include <numeric>
-#include <vector>
 
 namespace b200 {
 
@@ -256,53 +254,19 @@ void launch_level(int k, size_t smem, cudaStream_t st, const int32_t* s_uid, con
 
 using namespace b200;
 
-extern "C" int b200_nmf_prepare(const int32_t* indptr, const int32_t* indices, int64_t n_users, int64_t n_items,
-                                int64_t nnz, int32_t* csc_ptr, int32_t* csc_pos, int32_t* item_order)
+extern "C" int b200_nmf_fit(int64_t n_users, int64_t n_items, B200_SPARSE(r_, float), const int32_t* item_order,
+                            const int32_t* s_uid, const int32_t* s_iid, const float* s_rat, const int32_t* s_pos,
+                            const int32_t* level_ptr, int32_t n_levels, int k, float* U, float* V, float* Bu, float* Bi,
+                            float* rp, float* U_work, int n_epochs, float mu, float learning_rate, float lambda_u,
+                            float lambda_v, float lambda_bu, float lambda_bi, int use_bias, double* loss, void* stream)
 {
-    B200_REQUIRE(nnz >= 0 && nnz < (1ll << 31) && n_users >= 0 && n_items >= 0 && n_users < (1ll << 31) &&
-                     n_items < (1ll << 31),
-                 "b200_nmf_prepare: bad sizes n_users=%lld n_items=%lld nnz=%lld", (long long)n_users, (long long)n_items,
-                 (long long)nnz);
-    B200_REQUIRE(indptr && csc_ptr && item_order && (nnz == 0 || (indices && csc_pos)),
-                 "b200_nmf_prepare: null pointer argument");
-    B200_REQUIRE(indptr[0] == 0 && indptr[n_users] == nnz, "b200_nmf_prepare: indptr spans [%d, %d], expected [0, %lld]",
-                 indptr[0], indptr[n_users], (long long)nnz);
-    for (int64_t u = 0; u < n_users; ++u)
-        B200_REQUIRE(indptr[u] <= indptr[u + 1], "b200_nmf_prepare: indptr decreases at row %lld", (long long)u);
-    std::fill(csc_ptr, csc_ptr + n_items + 1, 0);
-    for (int64_t j = 0; j < nnz; ++j) {
-        const int32_t i = indices[j];
-        B200_REQUIRE(i >= 0 && i < n_items, "b200_nmf_prepare: rating %lld has item %d outside [0, %lld)", (long long)j, i,
-                     (long long)n_items);
-        ++csc_ptr[i + 1];
-    }
-    for (int64_t i = 0; i < n_items; ++i) csc_ptr[i + 1] += csc_ptr[i];
-    // counting sort: stable, so each column keeps the stored order of its ratings
-    std::vector<int32_t> next(csc_ptr, csc_ptr + n_items);
-    for (int64_t j = 0; j < nnz; ++j) csc_pos[next[indices[j]]++] = (int32_t)j;
-    std::iota(item_order, item_order + n_items, 0);
-    std::stable_sort(item_order, item_order + n_items, [&](int32_t a, int32_t b) {
-        return csc_ptr[a + 1] - csc_ptr[a] > csc_ptr[b + 1] - csc_ptr[b];
-    });
-    return B200_OK;
-}
-
-extern "C" int b200_nmf_fit(const int32_t* indptr, const int32_t* indices, const float* rating, int64_t n_users,
-                            int64_t n_items, int64_t nnz, const int32_t* csc_ptr, const int32_t* csc_row,
-                            const float* csc_val, const int32_t* csc_pos, const int32_t* item_order, const int32_t* s_uid,
-                            const int32_t* s_iid, const float* s_rat, const int32_t* s_pos, const int32_t* level_ptr,
-                            int32_t n_levels, int k, float* U, float* V, float* Bu, float* Bi, float* rp, float* U_work,
-                            int n_epochs, float mu, float learning_rate, float lambda_u, float lambda_v, float lambda_bu,
-                            float lambda_bi, int use_bias, double* loss, void* stream)
-{
-    B200_REQUIRE(k >= 1 && n_epochs >= 0 && n_users >= 0 && n_items >= 0 && nnz >= 0 && nnz < (1ll << 31) &&
-                     n_levels >= 0,
-                 "b200_nmf_fit: bad sizes k=%d n_epochs=%d n_users=%lld n_items=%lld nnz=%lld n_levels=%d", k, n_epochs,
-                 (long long)n_users, (long long)n_items, (long long)nnz, n_levels);
-    B200_REQUIRE(indptr && csc_ptr && item_order && U && V && Bu && Bi && U_work && U_work != U,
+    const SparseArgs<float> r = B200_SPARSE_VIEW(r_);
+    if (int rc = sparse_check(r, n_users, n_items, "b200_nmf_fit")) return rc;
+    const int64_t nnz = r.nnz;
+    B200_REQUIRE(k >= 1 && n_epochs >= 0 && n_levels >= 0, "b200_nmf_fit: bad sizes k=%d n_epochs=%d n_levels=%d", k,
+                 n_epochs, n_levels);
+    B200_REQUIRE(item_order && U && V && Bu && Bi && U_work && U_work != U && (nnz == 0 || rp),
                  "b200_nmf_fit: null or aliased pointer argument");
-    B200_REQUIRE(nnz == 0 || (indices && rating && csc_row && csc_val && csc_pos && rp),
-                 "b200_nmf_fit: null rating arrays");
     B200_REQUIRE(!use_bias || nnz == 0 || (s_uid && s_iid && s_rat && s_pos && level_ptr && n_levels > 0),
                  "b200_nmf_fit: use_bias needs the level schedule");
     if (n_epochs == 0 || n_users == 0 || n_items == 0) return B200_OK;
@@ -341,19 +305,19 @@ extern "C" int b200_nmf_fit(const int32_t* indptr, const int32_t* indices, const
             ::b200::count_launch();
         }
         if (k <= 32)
-            launch_user<1>(!bias_pass, grid_u, st, indptr, indices, rating, n_users, k, cur, V, Bu, Bi, mu, lambda_u, rp, nxt, le);
+            launch_user<1>(!bias_pass, grid_u, st, r.ptr, r.idx, r.val, n_users, k, cur, V, Bu, Bi, mu, lambda_u, rp, nxt, le);
         else if (k <= 64)
-            launch_user<2>(!bias_pass, grid_u, st, indptr, indices, rating, n_users, k, cur, V, Bu, Bi, mu, lambda_u, rp, nxt, le);
+            launch_user<2>(!bias_pass, grid_u, st, r.ptr, r.idx, r.val, n_users, k, cur, V, Bu, Bi, mu, lambda_u, rp, nxt, le);
         else
-            launch_user<4>(!bias_pass, grid_u, st, indptr, indices, rating, n_users, k, cur, V, Bu, Bi, mu, lambda_u, rp, nxt, le);
+            launch_user<4>(!bias_pass, grid_u, st, r.ptr, r.idx, r.val, n_users, k, cur, V, Bu, Bi, mu, lambda_u, rp, nxt, le);
         if (k <= 32)
-            nmf_item_kernel<1><<<grid_i, NMF_WARPS * 32, 0, st>>>(csc_ptr, csc_row, csc_val, csc_pos, item_order, n_items, k,
+            nmf_item_kernel<1><<<grid_i, NMF_WARPS * 32, 0, st>>>(r.cptr, r.crow, r.cval, r.cpos, item_order, n_items, k,
                                                                   cur, V, rp, lambda_v, le);
         else if (k <= 64)
-            nmf_item_kernel<2><<<grid_i, NMF_WARPS * 32, 0, st>>>(csc_ptr, csc_row, csc_val, csc_pos, item_order, n_items, k,
+            nmf_item_kernel<2><<<grid_i, NMF_WARPS * 32, 0, st>>>(r.cptr, r.crow, r.cval, r.cpos, item_order, n_items, k,
                                                                   cur, V, rp, lambda_v, le);
         else
-            nmf_item_kernel<4><<<grid_i, NMF_WARPS * 32, 0, st>>>(csc_ptr, csc_row, csc_val, csc_pos, item_order, n_items, k,
+            nmf_item_kernel<4><<<grid_i, NMF_WARPS * 32, 0, st>>>(r.cptr, r.crow, r.cval, r.cpos, item_order, n_items, k,
                                                                   cur, V, rp, lambda_v, le);
         ::b200::count_launch(2);
         B200_CUDA(cudaGetLastError());

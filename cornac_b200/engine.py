@@ -11,7 +11,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     pmf_schedule / pmf_fit         <-> pmf_linear / pmf_non_linear (cornac/models/pmf/cython/pmf.pyx:55-173)
     cofactor_schedule / cofactor_fit <-> sorec / mcf (cornac/models/sorec/cython/sorec.pyx, cornac/models/mcf/cython/mcf.pyx)
     score_batch_f64 / topk_rows_f64 <-> PMF.score / Recommender.rank (cornac/models/pmf/recom_pmf.py:191-222)
-    nmf_prepare / nmf_fit          <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
+    NmfData / nmf_fit              <-> NMF._fit_sgd          (cornac/models/nmf/recom_nmf.pyx:182-267)
     ease_fit / ease_score          <-> EASE.fit / EASE.score (cornac/models/ease/recom_ease.py:57-126)
     hpf_fit / hpf_update / hpf_expect <-> hpf_cpp / pf_cpp   (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275)
     c2pf_fit / c2pf_update  <-> c2pf_cpp / tc2pf_cpp / rc2pf_cpp  (cornac/models/c2pf/cpp/cpp_c2pf.cpp)
@@ -54,6 +54,11 @@ def to_device(a, dtype=None, pinned=True):
     if pinned:
         t = t.pin_memory()
     return t.cuda(non_blocking=True)
+
+
+def _pad(a):
+    """a, or one zero of its dtype when it is empty (no zero-size device buffers)."""
+    return a if len(a) else np.zeros(1, a.dtype)
 
 
 class BprData:
@@ -876,13 +881,12 @@ class CofactorData:
         self.n_levels = len(level_ptr) - 1
         o = self.order_host
         cat = lambda x, y, t: np.concatenate([np.asarray(x, dtype=t), np.asarray(y, dtype=t)])[o]   # noqa: E731
-        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)                                        # noqa: E731
-        self.a_id = to_device(pad(cat(net_a, uid, np.int32)), torch.int32)
-        self.b_id = to_device(pad(cat(net_b, iid, np.int32)), torch.int32)
-        self.val = to_device(pad(cat(net_val, rat, np.float32)), torch.float32)
-        self.is_edge = to_device(pad((o < self.n_edges).astype(np.uint8)), torch.uint8)
+        self.a_id = to_device(_pad(cat(net_a, uid, np.int32)), torch.int32)
+        self.b_id = to_device(_pad(cat(net_b, iid, np.int32)), torch.int32)
+        self.val = to_device(_pad(cat(net_val, rat, np.float32)), torch.float32)
+        self.is_edge = to_device(_pad((o < self.n_edges).astype(np.uint8)), torch.uint8)
         self.level_ptr = to_device(level_ptr, torch.int32)
-        self.order = to_device(pad(o), torch.int32)
+        self.order = to_device(_pad(o), torch.int32)
 
 
 def cofactor_fit(data, U, V, Z, cache_u, cache_v, cache_z, n_epochs, lambda_c, lambda_reg, learning_rate, gamma,
@@ -909,58 +913,74 @@ def cofactor_fit(data, U, V, Z, cache_u, cache_v, cache_z, n_epochs, lambda_c, l
                               ptr(data.order) if loss is not None else None, current_stream()), "b200_cofactor_fit")
 
 
-def nmf_prepare(indptr, indices, n_items):
-    """Host checks of the CSR ratings and NMF's stable CSC position map (b200_nmf_prepare, no device needed):
-    (csc_ptr int32 [n_items + 1], csc_pos int32 [nnz], item_order int32 [n_items]).  Column i lists the stored indices of
-    item i's ratings in stored order; item_order is the items by decreasing number of ratings."""
+def csc_map(indptr, indices, n_cols):
+    """Host checks of a CSR and its stable CSC position map (b200_csc_map, no device needed): (csc_ptr int32
+    [n_cols + 1], csc_pos int32 [nnz]); column c lists the CSR indices of its entries in stored order."""
     L = _lib.load()
     indptr = np.ascontiguousarray(indptr, dtype=np.int32)
     indices = np.ascontiguousarray(indices, dtype=np.int32)
-    nnz = len(indices)
-    csc_ptr = np.empty(int(n_items) + 1, dtype=np.int32)
-    csc_pos = np.empty(nnz, dtype=np.int32)
-    item_order = np.empty(int(n_items), dtype=np.int32)
-    check(L.b200_nmf_prepare(ptr(indptr), ptr(indices), len(indptr) - 1, int(n_items), nnz, ptr(csc_ptr), ptr(csc_pos),
-                             ptr(item_order)), "b200_nmf_prepare")
-    return csc_ptr, csc_pos, item_order
+    csc_ptr = np.empty(int(n_cols) + 1, dtype=np.int32)
+    csc_pos = np.empty(len(indices), dtype=np.int32)
+    check(L.b200_csc_map(ptr(indptr), ptr(indices), len(indptr) - 1, int(n_cols), len(indices), ptr(csc_ptr),
+                         ptr(csc_pos)), "b200_csc_map")
+    return csc_ptr, csc_pos
+
+
+def longest_first(lengths):
+    """The ids by decreasing length, ties in id order (int32): the order the fits launch their rows in."""
+    return np.argsort(-np.asarray(lengths), kind="stable").astype(np.int32)
+
+
+class SparseLayout:
+    """Device copy of an n_rows x n_cols sparse matrix, as B200_SPARSE (include/b200cornac.h) passes it: the CSR (ptr,
+    idx, val) with each entry's row, and its stable CSC transpose (csc_map) with the row, CSR index and value of each CSC
+    entry.  The values are stored as dtype (np.float32 or np.float64); col_lengths (host) counts each column's entries."""
+
+    def __init__(self, indptr, indices, values, n_cols, dtype):
+        require_cuda()
+        if len(indices) >= 2 ** 31:
+            raise B200Error("nnz >= 2^31 is not supported (int32 offsets)")
+        indptr = np.ascontiguousarray(indptr, dtype=np.int32)
+        indices = np.ascontiguousarray(indices, dtype=np.int32)
+        val = np.ascontiguousarray(values, dtype=dtype)
+        self.n_rows, self.n_cols, self.nnz = len(indptr) - 1, int(n_cols), len(indices)
+        if len(val) != self.nnz:
+            raise B200Error("%d values for %d entries" % (len(val), self.nnz))
+        cptr, cpos = csc_map(indptr, indices, self.n_cols)
+        row = np.repeat(np.arange(self.n_rows, dtype=np.int32), np.diff(indptr))
+        self.col_lengths = np.diff(cptr)
+        self.ptr, self.cptr = to_device(indptr), to_device(cptr)
+        self.idx, self.row, self.val = (to_device(_pad(a)) for a in (indices, row, val))
+        self.crow, self.cpos, self.cval = (to_device(_pad(a)) for a in (row[cpos], cpos, val[cpos]))
+
+    def args(self):
+        """The nine arguments of B200_SPARSE."""
+        return [ptr(self.ptr), ptr(self.idx), ptr(self.row), ptr(self.val), self.nnz, ptr(self.cptr), ptr(self.crow),
+                ptr(self.cpos), ptr(self.cval)]
 
 
 class NmfData:
-    """Device copy of NMF's ratings, built once per fit and used by every epoch: the CSR (indptr, indices, f32 ratings),
-    its stable CSC transpose (b200_nmf_prepare) and, only when the biases are trained, the ratings in the level order of
+    """Device copy of NMF's ratings, built once per fit and used by every epoch: the ratings as a SparseLayout (f32), the
+    items by decreasing number of ratings and, only when the biases are trained, the ratings in the level order of
     b200_pmf_schedule."""
 
     def __init__(self, indptr, indices, rating, n_items, use_bias):
-        require_cuda()
-        if len(indices) >= 2 ** 31:
-            raise B200Error("nnz >= 2^31 is not supported (int32 CSR offsets)")
-        indptr = np.ascontiguousarray(indptr, dtype=np.int32)
-        indices = np.ascontiguousarray(indices, dtype=np.int32)
-        rating = np.ascontiguousarray(rating, dtype=np.float32)
-        self.n_users, self.n_items, self.nnz = len(indptr) - 1, int(n_items), len(indices)
-        if len(rating) != self.nnz:
-            raise B200Error("rating has %d values for %d ratings" % (len(rating), self.nnz))
-        csc_ptr, csc_pos, item_order = nmf_prepare(indptr, indices, n_items)
-        uid = np.repeat(np.arange(self.n_users, dtype=np.int32), np.diff(indptr))
-        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
-        self.indptr = to_device(indptr, torch.int32)
-        self.indices = to_device(pad(indices), torch.int32)
-        self.rating = to_device(pad(rating), torch.float32)
-        self.csc_ptr = to_device(csc_ptr, torch.int32)
-        self.csc_pos = to_device(pad(csc_pos), torch.int32)
-        self.csc_row = to_device(pad(uid[csc_pos]), torch.int32)
-        self.csc_val = to_device(pad(rating[csc_pos]), torch.float32)
-        self.item_order = to_device(pad(item_order), torch.int32)
+        self.ratings = r = SparseLayout(indptr, indices, rating, n_items, np.float32)
+        self.n_users, self.n_items, self.nnz = r.n_rows, r.n_cols, r.nnz
+        self.item_order = to_device(_pad(longest_first(r.col_lengths)))
         self.use_bias = bool(use_bias)
         self.n_levels = 0
         self.s_uid = self.s_iid = self.s_rat = self.s_pos = self.level_ptr = None
         if self.use_bias:
+            uid = np.repeat(np.arange(self.n_users, dtype=np.int32), np.diff(indptr))
+            indices = np.asarray(indices, dtype=np.int32)
+            rating = np.asarray(rating, dtype=np.float32)
             order, level_ptr = pmf_schedule(uid, indices, self.n_users, self.n_items)
             self.n_levels = len(level_ptr) - 1
-            self.s_uid = to_device(pad(uid[order]), torch.int32)
-            self.s_iid = to_device(pad(indices[order]), torch.int32)
-            self.s_rat = to_device(pad(rating[order]), torch.float32)
-            self.s_pos = to_device(pad(order), torch.int32)
+            self.s_uid = to_device(_pad(uid[order]), torch.int32)
+            self.s_iid = to_device(_pad(indices[order]), torch.int32)
+            self.s_rat = to_device(_pad(rating[order]), torch.float32)
+            self.s_pos = to_device(_pad(order), torch.int32)
             self.level_ptr = to_device(level_ptr, torch.int32)
         self.rp = torch.empty(max(self.nnz, 1), dtype=torch.float32, device="cuda")
 
@@ -992,70 +1012,33 @@ def nmf_fit(data, U, V, Bu, Bi, n_epochs, mu=0.0, learning_rate=0.005, lambda_u=
     if workspace.numel() < U.numel() or workspace.data_ptr() == U.data_ptr():
         raise B200Error("workspace must hold U.numel() floats and must not alias U")
     f32 = lambda x: float(np.float32(x))              # noqa: E731
-    check(L.b200_nmf_fit(ptr(data.indptr), ptr(data.indices), ptr(data.rating), data.n_users, data.n_items, data.nnz,
-                         ptr(data.csc_ptr), ptr(data.csc_row), ptr(data.csc_val), ptr(data.csc_pos), ptr(data.item_order),
-                         ptr(data.s_uid), ptr(data.s_iid), ptr(data.s_rat), ptr(data.s_pos), ptr(data.level_ptr),
-                         data.n_levels, k, ptr(U), ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs),
-                         f32(mu), f32(learning_rate), f32(lambda_u), f32(lambda_v), f32(lambda_bu), f32(lambda_bi),
-                         int(data.use_bias), ptr(loss), current_stream()), "b200_nmf_fit")
-
-
-def efm_csc(indptr, indices, n_cols):
-    """Host checks of a CSR and its stable CSC position map (b200_efm_csc, no device needed): (csc_ptr int32
-    [n_cols + 1], csc_pos int32 [nnz]); column c lists the stored indices of its entries in stored order."""
-    L = _lib.load()
-    indptr = np.ascontiguousarray(indptr, dtype=np.int32)
-    indices = np.ascontiguousarray(indices, dtype=np.int32)
-    csc_ptr = np.empty(int(n_cols) + 1, dtype=np.int32)
-    csc_pos = np.empty(len(indices), dtype=np.int32)
-    check(L.b200_efm_csc(ptr(indptr), ptr(indices), len(indptr) - 1, int(n_cols), len(indices), ptr(csc_ptr),
-                         ptr(csc_pos)), "b200_efm_csc")
-    return csc_ptr, csc_pos
+    check(L.b200_nmf_fit(data.n_users, data.n_items, *data.ratings.args(), ptr(data.item_order), ptr(data.s_uid),
+                         ptr(data.s_iid), ptr(data.s_rat), ptr(data.s_pos), ptr(data.level_ptr), data.n_levels, k, ptr(U),
+                         ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs), f32(mu), f32(learning_rate),
+                         f32(lambda_u), f32(lambda_v), f32(lambda_bu), f32(lambda_bi), int(data.use_bias), ptr(loss),
+                         current_stream()), "b200_nmf_fit")
 
 
 class EfmData:
-    """Device copy of EFM's three matrices, built once per fit and used by every iteration: for each of A (users x
-    items), X (users x aspects) and Y (items x aspects) the CSR with each entry's row and its stable CSC transpose
-    (b200_efm_csc); the launch orders of the item and aspect rows (longest chains first); the prediction buffer."""
+    """Device copy of EFM's three matrices, built once per fit and used by every iteration: A (users x items), X (users x
+    aspects) and Y (items x aspects) as SparseLayouts (f32); the launch orders of the item and aspect rows (longest
+    chains first); the prediction buffer."""
 
     def __init__(self, A, X, Y):
-        require_cuda()
         A, X, Y = (_sp.csr_matrix(M) for M in (A, X, Y))
         self.n_users, self.n_items = A.shape
         self.n_aspects = X.shape[1]
         if X.shape[0] != self.n_users or Y.shape != (self.n_items, self.n_aspects):
             raise B200Error("A %s, X %s and Y %s do not agree in shape" % (A.shape, X.shape, Y.shape))
-        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
-        cols = {}
-        for name, M in (("a", A), ("x", X), ("y", Y)):
-            if M.nnz >= 2 ** 31:
-                raise B200Error("nnz >= 2^31 is not supported (int32 offsets)")
-            indptr = M.indptr.astype(np.int32)
-            indices = M.indices.astype(np.int32)
-            val = M.data.astype(np.float32)
-            row = np.repeat(np.arange(M.shape[0], dtype=np.int32), np.diff(indptr))
-            csc_ptr, csc_pos = efm_csc(indptr, indices, M.shape[1])
-            cols[name] = np.diff(csc_ptr)
-            setattr(self, "n" + name, int(M.nnz))
-            for field, a, dt in (("ptr", indptr, torch.int32), ("row", pad(row), torch.int32),
-                                 ("idx", pad(indices), torch.int32), ("val", pad(val), torch.float32),
-                                 ("cptr", csc_ptr, torch.int32), ("crow", pad(row[csc_pos]), torch.int32),
-                                 ("cpos", pad(csc_pos), torch.int32), ("cval", pad(val[csc_pos]), torch.float32)):
-                setattr(self, name + "_" + field, to_device(a, dt))
-        item_len = cols["a"] + np.diff(Y.indptr)
-        aspect_len = cols["x"] + cols["y"]
-        self.item_order = to_device(pad(np.argsort(-item_len, kind="stable").astype(np.int32)), torch.int32)
-        self.aspect_order = to_device(pad(np.argsort(-aspect_len, kind="stable").astype(np.int32)), torch.int32)
-        self.pred = torch.empty(max(self.na + self.nx + self.ny, 1), dtype=torch.float32, device="cuda")
+        self.a, self.x, self.y = (SparseLayout(M.indptr, M.indices, M.data, M.shape[1], np.float32) for M in (A, X, Y))
+        self.item_order = to_device(_pad(longest_first(self.a.col_lengths + np.diff(Y.indptr))))
+        self.aspect_order = to_device(_pad(longest_first(self.x.col_lengths + self.y.col_lengths)))
+        self.pred = torch.empty(max(self.a.nnz + self.x.nnz + self.y.nnz, 1), dtype=torch.float32, device="cuda")
 
     def args(self):
         """B200_EFM_DATA of include/b200cornac.h."""
-        out = []
-        for m in ("a", "x", "y"):
-            g = lambda f: getattr(self, m + "_" + f)                     # noqa: E731
-            out += [ptr(g("ptr")), ptr(g("row")), ptr(g("idx")), ptr(g("val")), getattr(self, "n" + m), ptr(g("cptr")),
-                    ptr(g("crow")), ptr(g("cpos")), ptr(g("cval"))]
-        return out + [ptr(self.item_order), ptr(self.aspect_order), self.n_users, self.n_items, self.n_aspects]
+        return self.a.args() + self.x.args() + self.y.args() + [ptr(self.item_order), ptr(self.aspect_order),
+                                                                  self.n_users, self.n_items, self.n_aspects]
 
 
 def efm_fit(data, U1, U2, V, H1, H2, n_iter, lambda_x=1.0, lambda_y=1.0, lambda_u=0.01, lambda_h=0.01, lambda_v=0.01,
@@ -1113,39 +1096,27 @@ def efm_queries(U1, H1, V, num_most_cared, alpha, rating_scale, user_idx=None):
     return Q
 
 
-class HpfData:
-    """Device copy of HPF's ratings, built once per fit and used by every iteration: the CSR (indptr, items, f64 values,
-    and each entry's user) and its CSC transpose (users ascending in each column) with the CSR index of each entry.
-    rid, cid, val: the stored (user, item, value) triplets, each pair at most once; zeros are the caller's to drop."""
+class HpfData(SparseLayout):
+    """Device copy of HPF's ratings, built once per fit and used by every iteration: a SparseLayout (f64) with items
+    ascending in each row, and the scratch of the fit.  rid, cid, val: the stored (user, item, value) triplets, each pair
+    at most once; zeros are the caller's to drop."""
 
     def __init__(self, rid, cid, val, n_users, n_items):
-        require_cuda()
         rid = np.asarray(rid, dtype=np.int64)
         cid = np.asarray(cid, dtype=np.int64)
         val = np.asarray(val, dtype=np.float64)
-        self.n_users, self.n_items, self.nnz = int(n_users), int(n_items), len(rid)
-        if len(cid) != self.nnz or len(val) != self.nnz:
-            raise B200Error("rid, cid and val differ in length (%d, %d, %d)" % (self.nnz, len(cid), len(val)))
-        if self.nnz >= 2 ** 31:
-            raise B200Error("nnz >= 2^31 is not supported (int32 offsets)")
-        if self.nnz and (rid.min() < 0 or rid.max() >= self.n_users or cid.min() < 0 or cid.max() >= self.n_items):
+        self.n_users, self.n_items, nnz = int(n_users), int(n_items), len(rid)
+        if len(cid) != nnz or len(val) != nnz:
+            raise B200Error("rid, cid and val differ in length (%d, %d, %d)" % (nnz, len(cid), len(val)))
+        if nnz and (rid.min() < 0 or rid.max() >= self.n_users or cid.min() < 0 or cid.max() >= self.n_items):
             raise B200Error("a rating lies outside the %d x %d matrix" % (self.n_users, self.n_items))
         order = np.lexsort((cid, rid))                       # CSR: users, then items ascending
         rid, cid, val = rid[order], cid[order], val[order]
-        if self.nnz > 1 and np.any((rid[1:] == rid[:-1]) & (cid[1:] == cid[:-1])):
+        if nnz > 1 and np.any((rid[1:] == rid[:-1]) & (cid[1:] == cid[:-1])):
             raise B200Error("a (user, item) pair is stored twice")
         indptr = np.zeros(self.n_users + 1, dtype=np.int64)
         np.cumsum(np.bincount(rid, minlength=self.n_users), out=indptr[1:])
-        csc_ptr, csc_pos, _ = nmf_prepare(indptr.astype(np.int32), cid.astype(np.int32), self.n_items)
-        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
-        self.indptr = to_device(indptr.astype(np.int32), torch.int32)
-        self.indices = to_device(pad(cid.astype(np.int32)), torch.int32)
-        self.row = to_device(pad(rid.astype(np.int32)), torch.int32)
-        self.val = to_device(pad(val), torch.float64)
-        self.csc_ptr = to_device(csc_ptr, torch.int32)
-        self.csc_pos = to_device(pad(csc_pos), torch.int32)
-        self.csc_row = to_device(pad(rid[csc_pos].astype(np.int32)), torch.int32)
-        self.csc_val = to_device(pad(val[csc_pos]), torch.float64)
+        super().__init__(indptr, cid, val, self.n_items, np.float64)
         self._work = {}
 
     def workspace(self, k):
@@ -1156,13 +1127,6 @@ class HpfData:
                 raise B200Error("bad HPF sizes")
             self._work = {k: torch.empty(nbytes // 8, dtype=torch.float64, device="cuda")}
         return self._work[k]
-
-    def args(self):
-        return (self.n_users, self.n_items, self.nnz)
-
-    def arrays(self):
-        return (ptr(self.indptr), ptr(self.indices), ptr(self.row), ptr(self.val), ptr(self.csc_ptr), ptr(self.csc_row),
-                ptr(self.csc_pos), ptr(self.csc_val))
 
 
 def _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr):
@@ -1187,8 +1151,9 @@ def hpf_fit(data, hierarchical, Gs, Gr, Ls, Lr, Kr, Tr, max_iter):
     k = _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr)
     if int(max_iter) < 0:
         raise B200Error("max_iter must be >= 0, got %d" % int(max_iter))
-    check(L.b200_hpf_fit(int(bool(hierarchical)), *data.args(), k, *data.arrays(), ptr(Gs), ptr(Gr), ptr(Ls), ptr(Lr),
-                         ptr(Kr), ptr(Tr), int(max_iter), ptr(data.workspace(k)), current_stream()), "b200_hpf_fit")
+    check(L.b200_hpf_fit(int(bool(hierarchical)), data.n_users, data.n_items, k, *data.args(), ptr(Gs), ptr(Gr), ptr(Ls),
+                         ptr(Lr), ptr(Kr), ptr(Tr), int(max_iter), ptr(data.workspace(k)), current_stream()),
+          "b200_hpf_fit")
 
 
 def hpf_update(data, hierarchical, Lt, Lb, Gs, Gr, Ls, Lr, Kr, Tr):
@@ -1199,8 +1164,8 @@ def hpf_update(data, hierarchical, Lt, Lb, Gs, Gr, Ls, Lr, Kr, Tr):
         _dev(t, torch.float64, name)
         if tuple(t.shape) != (rows, k):
             raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, k, tuple(t.shape)))
-    check(L.b200_hpf_update(int(bool(hierarchical)), *data.args(), k, *data.arrays(), ptr(Lt), ptr(Lb), ptr(Gs), ptr(Gr),
-                            ptr(Ls), ptr(Lr), ptr(Kr), ptr(Tr), ptr(data.workspace(k)), current_stream()),
+    check(L.b200_hpf_update(int(bool(hierarchical)), data.n_users, data.n_items, k, *data.args(), ptr(Lt), ptr(Lb),
+                            ptr(Gs), ptr(Gr), ptr(Ls), ptr(Lr), ptr(Kr), ptr(Tr), ptr(data.workspace(k)), current_stream()),
           "b200_hpf_update")
 
 
@@ -1242,12 +1207,11 @@ class C2pfGraph:
         if self.n_edges and (c_row.min() < 0 or c_row.max() >= d or c_mir.min() < 0 or c_mir.max() >= self.n_edges or
                              not np.array_equal(c_row[c_mir], c_col) or not np.array_equal(c_col[c_mir], c_row)):
             raise B200Error("c_mir does not map every entry (r, i) to a stored (i, r)")
-        pad = lambda a: a if len(a) else np.zeros(1, a.dtype)           # noqa: E731  (no zero-size device buffers)
         self.c_ptr = to_device(c_ptr.astype(np.int32), torch.int32)
-        self.c_row = to_device(pad(c_row.astype(np.int32)), torch.int32)
-        self.c_col = to_device(pad(c_col.astype(np.int32)), torch.int32)
-        self.c_mir = to_device(pad(c_mir.astype(np.int32)), torch.int32)
-        self.util = to_device(pad(np.asarray(util, dtype=np.float64)), torch.float64)
+        self.c_row = to_device(_pad(c_row.astype(np.int32)), torch.int32)
+        self.c_col = to_device(_pad(c_col.astype(np.int32)), torch.int32)
+        self.c_mir = to_device(_pad(c_mir.astype(np.int32)), torch.int32)
+        self.util = to_device(_pad(np.asarray(util, dtype=np.float64)), torch.float64)
         self._work = {}
 
     def workspace(self, k):
@@ -1282,8 +1246,8 @@ def _c2pf_args(graph, variant, at, bt, state):
         if t.numel() != size:
             raise B200Error("%s must hold %d values, got %d" % (name, size, t.numel()))
     ptrs = [None if name in absent else ptr(t) for t, name in zip(state[:6], names)] + [ptr(t) for t in state[6:]]
-    return k, [C2PF_VARIANTS[variant], *r.args(), k, *r.arrays(), graph.n_edges, ptr(graph.c_ptr), ptr(graph.c_row),
-               ptr(graph.c_col), ptr(graph.c_mir), ptr(graph.util), float(at), float(bt)] + ptrs
+    return k, [C2PF_VARIANTS[variant], r.n_users, r.n_items, k, *r.args(), graph.n_edges, ptr(graph.c_ptr),
+               ptr(graph.c_row), ptr(graph.c_col), ptr(graph.c_mir), ptr(graph.util), float(at), float(bt)] + ptrs
 
 
 def c2pf_fit(graph, variant, at, bt, state, n_iter):

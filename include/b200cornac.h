@@ -338,21 +338,31 @@ B200_API int b200_cofactor_fit(int variant, const int32_t* a_id, const int32_t* 
                                float gamma, double* loss, const int32_t* order, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * A sparse matrix (n_rows x n_cols, nnz stored entries) as NMF, HPF, C2PF and EFM take it, all on the device:
+ *   p##ptr, p##idx, p##row, p##val       the CSR int32[n_rows + 1] / int32[nnz] / int32[nnz] / T[nnz]: the row offsets,
+ *                                        then the column, row and value of each entry
+ *   p##cptr, p##crow, p##cpos, p##cval   its stable CSC transpose int32[n_cols + 1] / int32[nnz] / int32[nnz] / T[nnz]:
+ *                                        the column offsets, then the row, CSR index and value of each CSC entry
+ *
+ * b200_csc_map (HOST): checks a CSR (indptr int32[n_rows + 1] from 0 to nnz, never decreasing; indices int32[nnz] in
+ *   [0, n_cols)) and builds its stable CSC position map: csc_ptr int32[n_cols + 1] (column c is CSC entries
+ *   [csc_ptr[c], csc_ptr[c+1])) and csc_pos int32[nnz] (the CSR index of each CSC entry, stored order inside a column). */
+#define B200_SPARSE(p, T)                                                                                              \
+    const int32_t *p##ptr, const int32_t *p##idx, const int32_t *p##row, const T *p##val, int64_t p##nnz,              \
+        const int32_t *p##cptr, const int32_t *p##crow, const int32_t *p##cpos, const T *p##cval
+B200_API int b200_csc_map(const int32_t* indptr, const int32_t* indices, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                          int32_t* csc_ptr, int32_t* csc_pos);
+
+/* ------------------------------------------------------------------------------------
  * NMF (cornac/models/nmf/recom_nmf.pyx:182-267), multiplicative updates in plain IEEE f32, bit-identical to the
  * reference's serial loop.  Per epoch: a pass over the ratings in stored (CSR) order computes each prediction rp and,
  * with use_bias, steps the biases; then U and V are updated element-wise from ordered sums over each user's row and each
  * item's column (r * other factor and rp * other factor), the item sums reading the U the epoch started with.
  *
- * b200_nmf_prepare (HOST): checks the CSR (indptr int32[n_users + 1], indices int32[nnz]: every item in [0, n_items))
- * and builds the stable CSC position map:
- *   csc_ptr     host int32[n_items + 1]: column i is CSC entries [csc_ptr[i], csc_ptr[i+1])
- *   csc_pos     host int32[nnz]: the stored index of each CSC entry; stored order inside a column
- *   item_order  host int32[n_items]: items by decreasing number of ratings (ties by id), the order columns are launched in
- *
  * b200_nmf_fit: n_epochs epochs; calling it twice with a and b epochs is the same as calling it once with a + b.
- *   indptr, indices, rating   device CSR int32 / int32 / f32
- *   csc_ptr, csc_pos, item_order   device copies of b200_nmf_prepare's output
- *   csc_row, csc_val          device int32 / f32 [nnz]: the user and rating of each CSC entry
+ *   r_*                       the ratings, B200_SPARSE of f32 (n_users x n_items)
+ *   item_order                device int32[n_items]: items by decreasing number of ratings (ties by id), the order
+ *                             columns are launched in
  *   s_uid, s_iid, s_rat, s_pos, level_ptr, n_levels   with use_bias (else NULL / 0): the ratings in the level order of
  *                             b200_pmf_schedule (applied to the stored order), s_pos = their stored indices
  *   U, V, Bu, Bi              device f32 [n_users, k] / [n_items, k] / [n_users] / [n_items], updated in place; Bu and
@@ -362,11 +372,8 @@ B200_API int b200_cofactor_fit(int variant, const int32_t* a_id, const int32_t* 
  *   mu, learning_rate, lambda_*   f32, as the reference's `floating` locals
  *   loss                      device f64 [n_epochs] or NULL: += sum err^2 + lambda_u |U|^2 + lambda_v |V|^2 per epoch,
  *                             summed in f64 in no fixed order (a progress figure; not the reference's f32 sum)      */
-B200_API int b200_nmf_prepare(const int32_t* indptr, const int32_t* indices, int64_t n_users, int64_t n_items, int64_t nnz,
-                              int32_t* csc_ptr, int32_t* csc_pos, int32_t* item_order);
-B200_API int b200_nmf_fit(const int32_t* indptr, const int32_t* indices, const float* rating, int64_t n_users,
-                          int64_t n_items, int64_t nnz, const int32_t* csc_ptr, const int32_t* csc_row, const float* csc_val,
-                          const int32_t* csc_pos, const int32_t* item_order, const int32_t* s_uid, const int32_t* s_iid,
+B200_API int b200_nmf_fit(int64_t n_users, int64_t n_items, B200_SPARSE(r_, float), const int32_t* item_order,
+                          const int32_t* s_uid, const int32_t* s_iid,
                           const float* s_rat, const int32_t* s_pos, const int32_t* level_ptr, int32_t n_levels, int k,
                           float* U, float* V, float* Bu, float* Bi, float* rp, float* U_work, int n_epochs, float mu,
                           float learning_rate, float lambda_u, float lambda_v, float lambda_bu, float lambda_bi,
@@ -417,11 +424,7 @@ B200_API int b200_ease_score(const int64_t* users, int64_t n_q, int64_t n_items,
  * Every product, sum and quotient of the update is rounded on its own (no FMA) in the reference's order, so
  * b200_hpf_update is a fixed function of its inputs; the expectations use CUDA's exp / log and a Cephes digamma.
  *
- * The ratings (n_users x n_items, nnz stored values, no explicit zeros):
- *   indptr, indices, val     device CSR int32[n_users + 1] / int32[nnz] / f64[nnz], items ascending in each row
- *   row                      device int32[nnz]: the user of each CSR entry
- *   csc_ptr, csc_row, csc_pos, csc_val   device CSC int32[n_items + 1] / int32[nnz] / int32[nnz] / f64[nnz], users
- *                            ascending in each column; csc_pos = the CSR index of each CSC entry
+ * The ratings r_*: B200_SPARSE of f64 (n_users x n_items, no explicit zeros), items ascending in each row.
  * The state, device f64, updated in place: Gs, Gr [n_users, k]; Ls, Lr [n_items, k]; Kr [n_users]; Tr [n_items].
  * work: device scratch of b200_hpf_workspace_bytes(n_users, n_items, nnz, k) bytes.
  *
@@ -434,15 +437,12 @@ B200_API int b200_ease_score(const int64_t* users, int64_t n_q, int64_t n_items,
  *   iteration leaves, so two calls of a and b iterations equal one call of a + b.                                       */
 B200_API int64_t b200_hpf_workspace_bytes(int64_t n_users, int64_t n_items, int64_t nnz, int k);
 B200_API int b200_hpf_expect(const double* shape, const double* rate, int64_t n, double* out, void* stream);
-B200_API int b200_hpf_update(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k, const int32_t* indptr,
-                             const int32_t* indices, const int32_t* row, const double* val, const int32_t* csc_ptr,
-                             const int32_t* csc_row, const int32_t* csc_pos, const double* csc_val, const double* Lt,
-                             const double* Lb, double* Gs, double* Gr, double* Ls, double* Lr, double* Kr, double* Tr,
-                             double* work, void* stream);
-B200_API int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, int64_t nnz, int k, const int32_t* indptr,
-                          const int32_t* indices, const int32_t* row, const double* val, const int32_t* csc_ptr,
-                          const int32_t* csc_row, const int32_t* csc_pos, const double* csc_val, double* Gs, double* Gr,
-                          double* Ls, double* Lr, double* Kr, double* Tr, int max_iter, double* work, void* stream);
+B200_API int b200_hpf_update(int hierarchical, int64_t n_users, int64_t n_items, int k, B200_SPARSE(r_, double),
+                             const double* Lt, const double* Lb, double* Gs, double* Gr, double* Ls, double* Lr, double* Kr,
+                             double* Tr, double* work, void* stream);
+B200_API int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, int k, B200_SPARSE(r_, double), double* Gs,
+                          double* Gr, double* Ls, double* Lr, double* Kr, double* Tr, int max_iter, double* work,
+                          void* stream);
 
 /* ------------------------------------------------------------------------------------
  * C2PF (cornac/models/c2pf/cpp/cpp_c2pf.cpp): the variational fit of Collaborative Context Poisson Factorization in f64,
@@ -465,11 +465,10 @@ B200_API int b200_hpf_fit(int hierarchical, int64_t n_users, int64_t n_items, in
  *   iterations, enqueued without a host synchronisation.  Two calls of a and b iterations with the same (at, bt) equal
  *   one call of a + b.                                                                                                 */
 #define B200_C2PF_PARAMS                                                                                               \
-    int variant, int64_t n_users, int64_t n_items, int64_t nnz, int k, const int32_t *indptr, const int32_t *indices,  \
-        const int32_t *row, const double *val, const int32_t *csc_ptr, const int32_t *csc_row, const int32_t *csc_pos, \
-        const double *csc_val, int64_t n_edges, const int32_t *c_ptr, const int32_t *c_row, const int32_t *c_col,      \
-        const int32_t *c_mir, const double *util, double at, double bt, double *Gs, double *Gr, double *Ls, double *Lr, \
-        double *L2s, double *L2r, double *L3s, double *L3r, double *T3r
+    int variant, int64_t n_users, int64_t n_items, int k, B200_SPARSE(r_, double), int64_t n_edges,                    \
+        const int32_t *c_ptr, const int32_t *c_row, const int32_t *c_col, const int32_t *c_mir, const double *util,    \
+        double at, double bt, double *Gs, double *Gr, double *Ls, double *Lr, double *L2s, double *L2r, double *L3s,   \
+        double *L3r, double *T3r
 B200_API int64_t b200_c2pf_workspace_bytes(int64_t n_users, int64_t n_items, int64_t nnz, int64_t n_edges, int k);
 B200_API int b200_c2pf_update(B200_C2PF_PARAMS, double* Lt, double* Lb, double* L2b, double* L3b, double* Lb2,
                               const double* given_Lt, const double* given_Lb, const double* given_L2b,
@@ -483,19 +482,15 @@ B200_API int b200_c2pf_fit(B200_C2PF_PARAMS, int n_iter, double* work, void* str
  * once to f32; the A prediction f32(U1.U2) + f32(H1.H2)); everything else is the reference's f32 arithmetic and order,
  * so the fit is bit-identical to oracle/efm_oracle.c.  Every accumulator reads the factors the iteration started with.
  *
- * b200_efm_csc (HOST): checks a CSR (indptr int32[n_rows + 1], indices int32[nnz] in [0, n_cols)) and builds its stable
- *   CSC position map: csc_ptr int32[n_cols + 1], csc_pos int32[nnz] (the stored index of each CSC entry, stored order
- *   inside a column).
- *
  * b200_efm_fit: n_iter iterations; two calls of a and b iterations equal one call of a + b.  B200_EFM_DATA, all device:
- *   m_ptr, m_row, m_idx, m_val       the CSR of m = a, x, y (m_row: the row of each entry), nM entries
- *   m_cptr, m_crow, m_cpos, m_cval   its CSC (b200_efm_csc): the row, stored index and value of each CSC entry
+ *   a_*, x_*, y_*  the matrices A, X and Y, each a B200_SPARSE of f32
  *   item_order    int32[n_items]: the order item rows are launched in (longest chains first)
  *   aspect_order  int32[n_aspects]: the order aspect rows are launched in (longest chains first)
  * U1 [n_users, E], U2 [n_items, E], V [n_aspects, E], H1 [n_users, L], H2 [n_items, L]: device f32, updated in place.
- * work: device f32 workspace of (n_users + n_items) * (E + L) + n_aspects * E floats; pred: device f32 [nA + nX + nY]
- * (the last iteration's predictions on return).  lambda_*: f32, as the reference's `floating` locals.  loss: device f64
- * [n_iter] or NULL: += the reference's loss terms of each iteration, summed in f64 in no fixed order.
+ * work: device f32 workspace of (n_users + n_items) * (E + L) + n_aspects * E floats; pred: device f32
+ * [a_nnz + x_nnz + y_nnz] (the last iteration's predictions on return).  lambda_*: f32, as the reference's `floating`
+ * locals.  loss: device f64 [n_iter] or NULL: += the reference's loss terms of each iteration, summed in f64 in no fixed
+ * order.
  *
  * b200_efm_queries: the query vector of each user users[q] (device int64[n_q]) for the aspect-weighted rank:
  *   X_[a] = dot(U1[u], V[a]) (the defined dot); a_0..a_{m-1} the m = min(N, n_aspects) aspects of largest X_ (ties: the
@@ -505,15 +500,8 @@ B200_API int b200_c2pf_fit(B200_C2PF_PARAMS, int n_iter, double* work, void* str
  *   Q[q] . [U2 | H2][i] is, up to rounding, alpha * explicit(u, i) + (1 - alpha) * score(u, i): the row the reference's
  *   rank() orders.                                                                                                      */
 #define B200_EFM_DATA                                                                                                   \
-    const int32_t *a_ptr, const int32_t *a_row, const int32_t *a_idx, const float *a_val, int64_t nA,                   \
-        const int32_t *a_cptr, const int32_t *a_crow, const int32_t *a_cpos, const float *a_cval, const int32_t *x_ptr,  \
-        const int32_t *x_row, const int32_t *x_idx, const float *x_val, int64_t nX, const int32_t *x_cptr,              \
-        const int32_t *x_crow, const int32_t *x_cpos, const float *x_cval, const int32_t *y_ptr, const int32_t *y_row,   \
-        const int32_t *y_idx, const float *y_val, int64_t nY, const int32_t *y_cptr, const int32_t *y_crow,             \
-        const int32_t *y_cpos, const float *y_cval, const int32_t *item_order, const int32_t *aspect_order,             \
-        int64_t n_users, int64_t n_items, int64_t n_aspects
-B200_API int b200_efm_csc(const int32_t* indptr, const int32_t* indices, int64_t n_rows, int64_t n_cols, int64_t nnz,
-                          int32_t* csc_ptr, int32_t* csc_pos);
+    B200_SPARSE(a_, float), B200_SPARSE(x_, float), B200_SPARSE(y_, float), const int32_t *item_order,                  \
+        const int32_t *aspect_order, int64_t n_users, int64_t n_items, int64_t n_aspects
 B200_API int b200_efm_fit(B200_EFM_DATA, int E, int L, float* U1, float* U2, float* V, float* H1, float* H2, float* work,
                           float* pred, int n_iter, float lambda_x, float lambda_y, float lambda_u, float lambda_h,
                           float lambda_v, double* loss, void* stream);

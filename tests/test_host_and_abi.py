@@ -15,7 +15,7 @@ def _product():
     return _lib
 
 
-def test_library_loads_and_exports_every_declared_symbol():
+def test_library_loads_and_exports_every_declared_symbol_of_abi_3():
     _lib = _product()
     L = _lib.load()
     header = open(os.path.join(ROOT, "include", "b200cornac.h")).read()
@@ -24,7 +24,7 @@ def test_library_loads_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(L, name), "include/b200cornac.h declares %s but the library does not export it" % name
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
-    assert L.b200_abi_version() == 2 and L.b200_kernel_launches() >= 0
+    assert L.b200_abi_version() == 3 and L.b200_kernel_launches() >= 0
 
 
 def test_sampler_matches_oracle_streams():

@@ -36,11 +36,11 @@ def test_fixtures_cover_the_cases():
 
 
 @pytest.mark.parametrize("shape", [(1, 1, 1), (30, 20, 300), (943, 1682, 20000)])
-def test_csc_map_is_a_stable_permutation(shape):
+def test_b200_csc_map_is_a_stable_permutation(shape):
     from cornac_b200 import engine
     n_users, n_items, nnz = shape
     indptr, indices = synth_csr(n_users, n_items, nnz, seed=nnz)
-    csc_ptr, csc_pos, item_order = engine.nmf_prepare(indptr, indices, n_items)
+    csc_ptr, csc_pos = engine.csc_map(indptr, indices, n_items)
     n = len(indices)
     assert np.array_equal(np.sort(csc_pos), np.arange(n))
     assert np.array_equal(np.diff(csc_ptr), np.bincount(indices, minlength=n_items))
@@ -49,19 +49,21 @@ def test_csc_map_is_a_stable_permutation(shape):
         assert np.all(indices[col] == i) and np.all(np.diff(col) > 0)
     assert np.array_equal(csc_pos, np.argsort(indices, kind="stable"))
     deg = np.diff(csc_ptr)
-    assert np.array_equal(item_order, np.lexsort((np.arange(n_items), -deg)))
+    item_order = engine.longest_first(deg)
+    assert item_order.dtype == np.int32 and np.array_equal(item_order, np.lexsort((np.arange(n_items), -deg)))
 
 
-def test_prepare_rejects_bad_input():
+def test_csc_map_rejects_bad_input():
     from cornac_b200 import engine
     from cornac_b200._lib import B200Error
     with pytest.raises(B200Error, match="outside"):
-        engine.nmf_prepare(np.array([0, 2]), np.array([0, 3]), 3)
+        engine.csc_map(np.array([0, 2]), np.array([0, 3]), 3)
     with pytest.raises(B200Error, match="indptr"):
-        engine.nmf_prepare(np.array([0, 3]), np.array([0, 1]), 3)
+        engine.csc_map(np.array([0, 3]), np.array([0, 1]), 3)
     with pytest.raises(B200Error, match="decreases"):
-        engine.nmf_prepare(np.array([0, 2, 1, 2]), np.array([0, 1]), 3)
-    ptr_, pos, order = engine.nmf_prepare(np.zeros(1), np.zeros(0), 0)
+        engine.csc_map(np.array([0, 2, 1, 2]), np.array([0, 1]), 3)
+    ptr_, pos = engine.csc_map(np.zeros(1), np.zeros(0), 0)
+    order = engine.longest_first(np.diff(ptr_))
     assert list(ptr_) == [0] and len(pos) == 0 and len(order) == 0
 
 
