@@ -9,7 +9,7 @@ Layers:  include/b200cornac.h (C ABI)  <-  cornac_b200/csrc (CUDA)  <-  cornac_b
 plug-ins).  The plug-in classes need the `cornac` package importable (they subclass its
 Recommender so that cornac.Experiment accepts them); the engine does not.
 """
-__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "HPF", "SoRec", "MCF", "C2PF", "EFM", "engine", "B200Error"]
+__all__ = ["BPR", "WBPR", "MMMF", "VEBPR", "SBPR", "MF", "WMF", "BaselineOnly", "UserKNN", "ItemKNN", "PMF", "NMF", "EASE", "HPF", "SoRec", "MCF", "C2PF", "EFM", "MTER", "engine", "B200Error"]
 
 from ._lib import B200Error  # noqa: F401
 
@@ -63,6 +63,9 @@ def __getattr__(name):
     if name == "EFM":
         from .recom_efm import EFM
         return EFM
+    if name == "MTER":
+        from .recom_mter import MTER
+        return MTER
     if name == "BaselineOnly":
         from .recom_bo import BaselineOnly
         return BaselineOnly

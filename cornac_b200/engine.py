@@ -16,7 +16,10 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     hpf_fit / hpf_update / hpf_expect <-> hpf_cpp / pf_cpp   (cornac/models/hpf/cpp/cpp_hpf.cpp:139-275)
     c2pf_fit / c2pf_update  <-> c2pf_cpp / tc2pf_cpp / rc2pf_cpp  (cornac/models/c2pf/cpp/cpp_c2pf.cpp)
     efm_fit / efm_queries   <-> EFM._fit_efm / EFM.rank  (cornac/models/efm/recom_efm.pyx:268-353, 471-528)
+    mter_fit / mter_queries <-> MTER._fit_mter / MTER.score (cornac/models/mter/recom_mter.pyx:434-714)
 """
+import ctypes
+
 import numpy as np
 import scipy.sparse as _sp
 import torch
@@ -1093,6 +1096,154 @@ def efm_queries(U1, H1, V, num_most_cared, alpha, rating_scale, user_idx=None):
     check(L_.b200_efm_queries(ptr(user_idx), user_idx.numel(), ptr(U1), ptr(H1), ptr(V), int(V.shape[0]), E, Lw,
                               int(num_most_cared), float(alpha), float(rating_scale), ptr(Q), current_stream()),
           "b200_efm_queries")
+    return Q
+
+
+MTER_PARAMS = ("U", "I", "A", "O", "G1", "G2", "G3")
+_MTER_DRAW_CHUNK = 1 << 24        # draws uploaded per chunk (64 MB of int32)
+
+
+class MterData:
+    """The arrays `fit` hands to `_fit_mter` (recom_mter.pyx:334-371), in the reference's order.
+
+    X, YU, YI: f32 values; X_uids / X_iids / X_aids, YU_uids / YU_aids / YU_oids, YI_iids / YI_aids / YI_oids: int32
+    indices.  indptr / indices: the rating CSR (sorted columns; repeated pairs summed, as scipy builds it); user_ids:
+    the row of each CSR entry; pair_rating: the f32 rating of each entry's exact (user, item) pair, the last value a
+    repeated pair has (what the reference's IntFloatDict keeps) -- the BPR skip and sign rule reads it."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+class MterDraws:
+    """The five seeded sample streams, drawn on the host in chunks of iterations and uploaded through two pinned
+    buffers: chunk k + 1 is drawn while the GPU runs chunk k."""
+
+    def __init__(self, seeds, data, n_el, n_bpr, max_chunk):
+        self.samplers = [MTSampler(s) for s in seeds]
+        self.hi = [len(data.X) - 1, len(data.YU) - 1, len(data.YI) - 1, len(data.indices) - 1, data.n_items - 1]
+        self.n = [n_el, n_el, n_el, n_bpr, n_bpr]
+        self.per_iter = 3 * n_el + 2 * n_bpr
+        self.chunk = max(1, min(int(max_chunk), _MTER_DRAW_CHUNK // self.per_iter))
+        self.host = [torch.empty((self.chunk, self.per_iter), dtype=torch.int32).pin_memory() for _ in range(2)]
+        self.dev = [torch.empty((self.chunk, self.per_iter), dtype=torch.int32, device="cuda") for _ in range(2)]
+        self.done = [None, None]
+        self.slot = 0
+
+    def draw(self, n_iter):
+        """Draws of the next n_iter iterations as one int64 array [n_iter, per_iter]."""
+        cols = [s.fill(h, n_iter * n).reshape(n_iter, n) for s, h, n in zip(self.samplers, self.hi, self.n)]
+        return np.concatenate(cols, axis=1)
+
+    def next(self, n_iter):
+        """Device draws of the next n_iter (<= chunk) iterations."""
+        k = self.slot
+        self.slot ^= 1
+        if self.done[k] is not None:
+            self.done[k].synchronize()                 # the last upload from this pinned buffer has finished
+        host = self.host[k][:n_iter]
+        host.numpy()[:] = self.draw(n_iter)
+        dev = self.dev[k][:n_iter]
+        dev.copy_(host, non_blocking=True)
+        self.done[k] = torch.cuda.Event()
+        self.done[k].record()
+        return dev
+
+
+class MterDeviceData:
+    """Device copy of MTER's training data (a recom_mter.MterData): the three sentiment tensors and the ratings' CSR
+    with each entry's row and pair rating, uploaded once per fit."""
+
+    def __init__(self, data):
+        i32 = lambda a: to_device(_pad(np.asarray(a, dtype=np.int32)), torch.int32)      # noqa: E731
+        f32 = lambda a: to_device(_pad(np.asarray(a, dtype=np.float32)), torch.float32)  # noqa: E731
+        self.n_users, self.n_items = int(data.n_users), int(data.n_items)
+        self.n_aspects, self.n_opinions = int(data.n_aspects), int(data.n_opinions)
+        self.x = [f32(data.X), i32(data.X_uids), i32(data.X_iids), i32(data.X_aids)]
+        self.yu = [f32(data.YU), i32(data.YU_uids), i32(data.YU_aids), i32(data.YU_oids)]
+        self.yi = [f32(data.YI), i32(data.YI_iids), i32(data.YI_aids), i32(data.YI_oids)]
+        self.n_x, self.n_yu, self.n_yi = len(data.X), len(data.YU), len(data.YI)
+        self.csr = [i32(data.indptr), i32(data.indices), i32(data.user_ids), f32(data.pair_rating)]
+        self.nnz = len(data.indices)
+
+    def args(self):
+        return [self.n_users, self.n_items, self.n_aspects, self.n_opinions]
+
+
+def mter_workspace_bytes(data, dims, n_el, n_bpr):
+    L_ = require_cuda()
+    return int(L_.b200_mter_workspace_bytes(data.n_users, data.n_items, data.n_aspects, data.n_opinions, *dims,
+                                            int(n_el), int(n_bpr)))
+
+
+def mter_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, lr=0.1, lambda_reg=0.1, lambda_bpr=10.0, counts=None,
+             losses=None, workspace=None, unordered=False, philox_seed=None, iter0=0, phase_ns=None):
+    """n_iter iterations of MTER._fit_mter (recom_mter.pyx:434-675) over `data` (MterDeviceData), bit for bit as the
+    reference's serial f32 loop given the draws.  params / sgrad: sequences of the f32 device tensors U, I, A, O, G1,
+    G2, G3 and their AdaGrad sums, updated in place.  draws: int32 device tensor [n_iter, 3 n_el + 2 n_bpr] (per
+    iteration the uia, uao, iao, pos and neg draws).  counts: int64 device [2] (+= correct, skipped).  losses: f64
+    device [2] or None (+= loss, bpr_loss, summed in f64).  workspace: uint8 device tensor of mter_workspace_bytes
+    that is zero before its first use (the fit leaves the part it needs zero); allocated per call when None.
+    unordered: sum the rows' gradients per sample with f32 atomics (no fixed order).  philox_seed: draw on the device
+    from Philox4x32-10 with this key, iterations iter0, iter0 + 1, ... (draws is then ignored and may be None).
+    phase_ns: int64 device [4] or None (+= nanoseconds of the predictions, owners + stored terms, gradients, AdaGrad)."""
+    L_ = require_cuda()
+    U, I, A, O, G1, G2, G3 = params
+    dims = (int(G1.shape[0]), int(G1.shape[1]), int(G2.shape[1]), int(G2.shape[2]))
+    d1, d2, d3, d4 = dims
+    shapes = ((data.n_users, d1), (data.n_items, d2), (data.n_aspects + 1, d3), (data.n_opinions, d4), (d1, d2, d3),
+              (d1, d3, d4), (d2, d3, d4))
+    for name, t, st, shape in zip(MTER_PARAMS, params, sgrad, shapes):
+        _dev(t, torch.float32, name), _dev(st, torch.float32, "sgrad_" + name)
+        if tuple(t.shape) != shape or tuple(st.shape) != shape:
+            raise B200Error("%s and its AdaGrad sum must have shape %s, got %s / %s"
+                            % (name, shape, tuple(t.shape), tuple(st.shape)))
+    per_iter = 3 * int(n_el) + 2 * int(n_bpr)
+    if philox_seed is None:
+        _dev(draws, torch.int32, "draws")
+        if draws.numel() < int(n_iter) * per_iter:
+            raise B200Error("draws must hold n_iter * (3 n_el + 2 n_bpr) = %d values" % (int(n_iter) * per_iter))
+    else:
+        draws = None
+    if phase_ns is not None:
+        _dev(phase_ns, torch.int64, "phase_ns")
+    if counts is None:
+        counts = torch.zeros(2, dtype=torch.int64, device="cuda")
+    _dev(counts, torch.int64, "counts")
+    if losses is not None:
+        _dev(losses, torch.float64, "losses")
+    need = mter_workspace_bytes(data, dims, n_el, n_bpr)
+    if workspace is None:
+        workspace = torch.zeros(need, dtype=torch.uint8, device="cuda")
+    _dev(workspace, torch.uint8, "workspace")
+    if workspace.numel() < need:
+        raise B200Error("workspace must hold %d bytes" % need)
+    pp = (ctypes.c_void_p * 7)(*[ptr(t) for t in params])
+    ps = (ctypes.c_void_p * 7)(*[ptr(t) for t in sgrad])
+    f32 = lambda x: float(np.float32(x))              # noqa: E731
+    check(L_.b200_mter_fit(*data.args(), *dims, *[ptr(t) for t in data.x], data.n_x, *[ptr(t) for t in data.yu],
+                           data.n_yu, *[ptr(t) for t in data.yi], data.n_yi, *[ptr(t) for t in data.csr], data.nnz,
+                           int(n_el), int(n_bpr), int(n_iter), ptr(draws), pp, ps, ptr(workspace), f32(lr),
+                           f32(lambda_reg), f32(lambda_bpr),
+                           (_lib.MTER_UNORDERED if unordered else 0) | (0 if philox_seed is None else _lib.MTER_PHILOX),
+                           int(philox_seed or 0) & (2 ** 64 - 1), int(iter0), ptr(counts), ptr(losses), ptr(phase_ns),
+                           current_stream()),
+          "b200_mter_fit")
+    return counts
+
+
+def mter_queries(U, G1, A):
+    """[n_users, d2] f32 rank queries (b200_mter_queries): Q[u] . I[i] is MTER.score(u)[i] = einsum(G1, U[u], I[i],
+    A[-1]) up to rounding.  M = G1 . A[-1] and Q = U . M are f64 sums in index order, each rounded once to f32."""
+    L_ = require_cuda()
+    for t, name in ((U, "U"), (G1, "G1"), (A, "A")):
+        _dev(t, torch.float32, name)
+    d1, d2, d3 = (int(x) for x in G1.shape)
+    if U.dim() != 2 or int(U.shape[1]) != d1 or A.dim() != 2 or int(A.shape[1]) != d3 or A.shape[0] < 1:
+        raise B200Error("U %s, G1 %s and A %s do not agree in shape" % (tuple(U.shape), tuple(G1.shape), tuple(A.shape)))
+    Q = torch.empty((U.shape[0], d2), dtype=torch.float32, device=U.device)
+    check(L_.b200_mter_queries(ptr(U), int(U.shape[0]), ptr(G1), ptr(A[-1]), d1, d2, d3, ptr(Q), current_stream()),
+          "b200_mter_queries")
     return Q
 
 

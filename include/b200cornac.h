@@ -627,6 +627,53 @@ B200_API int b200_rank_counts(float* scores, int64_t n_q, int64_t n_items,
                               int64_t* less, float* pos_score, int64_t* n_cand, int64_t* before_first, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * MTER (cornac/models/mter/recom_mter.pyx:434-675): the seeded fit, bit-identical to the reference's serial f32 loop
+ * given the same draws.  Shapes: U [n_users, d1], I [n_items, d2], A [n_aspects + 1, d3],
+ * O [n_opinions, d4], G1 [d1, d2, d3], G2 [d1, d3, d4], G3 [d2, d3, d4], row-major device f32.
+ *
+ * b200_mter_fit: n_iter iterations in one cooperative launch; two calls of a and b iterations equal one call of a + b.
+ *   X / YU / YI       the three sentiment tensors: f32 values and int32 index arrays of n_x / n_yu / n_yi entries
+ *   indptr, indices   the CSR of the ratings (sorted columns), rrow the row of each entry, rval the f32 rating of
+ *                     the entry's exact (user, item) pair: the BPR skip / sign rule
+ *   draws             int32 [n_iter][3 n_el + 2 n_bpr]: per iteration the uia, uao, iao draws (n_el each), then the
+ *                     pos and neg draws (n_bpr each), as the reference's five RNGVector streams give them; unused (may
+ *                     be NULL) with B200_MTER_PHILOX
+ *   flags             0: the exact mode.  B200_MTER_PHILOX: draw k of iteration iter0 + it is Philox4x32-10 of
+ *                     (k, iteration) with key `seed`, reduced to [0, n) (bias <= n / 2^64), the reference's uniform law.
+ *                     B200_MTER_UNORDERED: the rows' gradients are summed per sample with f32 atomics (no fixed order;
+ *                     the result can differ from run to run by rounding) instead of the reference's ordered chains.
+ *                     Seeded fits use 0; unseeded fits both flags (the reference defines no order without a seed)
+ *   params, sgrad     host arrays of 7 device pointers in the order U, I, A, O, G1, G2, G3: the parameters and their
+ *                     AdaGrad sums, updated in place (the reference's del_*_reg is reset every iteration: no state)
+ *   work              device, b200_mter_workspace_bytes(...) bytes, zero before the first call; the fit leaves the
+ *                     part that must be zero (del and the row owners) zero
+ *   phase_ns          device u64[4] or NULL: += the nanoseconds of the phases (predictions, owners + stored terms,
+ *                     gradients, AdaGrad) as block 0 sees them
+ *   lr, lambda_*      f32, as the reference's `floating` locals
+ *   counts            device u64[2]: += correct, skipped over the call's iterations
+ *   losses            device f64[2] or NULL: += the squared errors and the BPR log-likelihood terms, summed in f64 in
+ *                     no fixed order (the reference's figures are f32 sums)
+ *
+ * b200_mter_queries: Q [n_users, d2] = the rank query of every user: M[p, q] = f32(sum_r G1[p, q, r] a_last[r]) and
+ *   Q[u, q] = f32(sum_p U[u, p] M[p, q]), each an f64 sum in index order of exact products.  Q . I[i] is score(u)[i]
+ *   up to rounding.                                                                                                    */
+#define B200_MTER_UNORDERED 1
+#define B200_MTER_PHILOX 2
+B200_API int64_t b200_mter_workspace_bytes(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions,
+                                           int d1, int d2, int d3, int d4, int n_el, int n_bpr);
+B200_API int b200_mter_fit(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1, int d2,
+                           int d3, int d4, const float* X, const int32_t* X_u, const int32_t* X_i, const int32_t* X_a,
+                           int64_t n_x, const float* YU, const int32_t* YU_u, const int32_t* YU_a, const int32_t* YU_o,
+                           int64_t n_yu, const float* YI, const int32_t* YI_i, const int32_t* YI_a, const int32_t* YI_o,
+                           int64_t n_yi, const int32_t* indptr, const int32_t* indices, const int32_t* rrow,
+                           const float* rval, int64_t nnz, int n_el, int n_bpr, int n_iter, const int32_t* draws,
+                           float* const* params, float* const* sgrad, void* work, float lr, float lambda_reg,
+                           float lambda_bpr, int flags, uint64_t seed, uint64_t iter0, unsigned long long* counts,
+                           double* losses, unsigned long long* phase_ns, void* stream);
+B200_API int b200_mter_queries(const float* U, int64_t n_users, const float* G1, const float* a_last, int d1, int d2,
+                               int d3, float* Q, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Multi-GPU item-factor exchange (no reference counterpart: the reference is a single
  * process).  Each rank trains its user shard against a replica of V / B; at the epoch
  * boundary   b200_delta_make:  delta[i] = x[i] - snapshot[i]
