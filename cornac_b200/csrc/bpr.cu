@@ -852,6 +852,7 @@ struct DetState {
     DetPlan plan[2];                // by round parity
     unsigned long long* acc;        // [cap][k + 1] 2^-40 fixed-point sums of the shared rows; column k = the item bias
     unsigned int* n_shared;         // [rounds] slots taken by each round
+    unsigned int cap;               // slots of a round's row_of_slot
     float d_max;                    // bound on |d| that keeps every round sum in range (det_delta_bound)
 };
 
@@ -963,7 +964,10 @@ __device__ __forceinline__ DetDst det_dst(float* x, const unsigned int* cnt, con
                                           unsigned long long* acc, int k)
 {
     DetDst t{x, nullptr};
-    if (__ldcg(cnt + row) >= 2u) t.a = acc + (size_t)__ldcg(slot + row) * (size_t)(k + 1);
+    // the slot is read beside the count, not after it: one round trip (a row touched once has a stale or unset slot,
+    // which is not used)
+    const unsigned c = __ldcg(cnt + row), s = __ldcg(slot + row);
+    if (c >= 2u) t.a = acc + (size_t)s * (size_t)(k + 1);
     return t;
 }
 
@@ -1077,15 +1081,23 @@ __global__ void __launch_bounds__(256) bpr_det_apply_kernel(const BprParams p, c
     }
     det_pdl_sync();
     const DetPlan pl = par ? d.plan[1] : d.plan[0];
-    const unsigned n_sh = __ldcg(d.n_shared + r);
     const int k = p.k;
     const unsigned n_warps = gridDim.x * (blockDim.x / 32);
-    for (unsigned s = (unsigned)(t / 32); s < n_sh; s += n_warps) {
-        const unsigned tag = __ldcg(pl.row_of_slot + s);
+    // the warp's first slot's row is read beside the round's slot count, before it is known to be one of the round's
+    const unsigned s0 = (unsigned)(t / 32);
+    unsigned tag = s0 < d.cap ? __ldcg(pl.row_of_slot + s0) : 0u;
+    const unsigned n_sh = __ldcg(d.n_shared + r);
+    for (unsigned s = s0; s < n_sh; s += n_warps) {
+        if (s != s0) tag = __ldcg(pl.row_of_slot + s);
         const int32_t row = (int32_t)(tag & ~DET_ITEM);
         const bool item = tag & DET_ITEM;
         float* x = (item ? p.V : p.U) + (size_t)row * k;
         unsigned long long* a = d.acc + (size_t)s * (size_t)(k + 1);
+        // the bias sum and value are read with the first elements
+        const bool bias = lane == 0 && item && p.use_bias;
+        long long qb = 0;
+        float vb = 0.f;
+        if (bias) { qb = (long long)__ldcg(a + k); vb = __ldcg(p.B + row); }
         for (int e0 = 0; e0 < k; e0 += 32 * DET_RC) {       // DET_RC elements per lane in flight at once
             long long q[DET_RC];
             float v[DET_RC];
@@ -1101,10 +1113,8 @@ __global__ void __launch_bounds__(256) bpr_det_apply_kernel(const BprParams p, c
                 if (e < k) det_apply(a + e, x + e, q[c], v[c]);
             }
         }
-        if (lane == 0) {
-            if (item && p.use_bias) det_apply(a + k, p.B + row, (long long)__ldcg(a + k), __ldcg(p.B + row));
-            (item ? pl.cnt_v : pl.cnt_u)[row] = 0u;
-        }
+        if (bias) det_apply(a + k, p.B + row, qb, vb);
+        if (lane == 0) (item ? pl.cnt_v : pl.cnt_u)[row] = 0u;
     }
 }
 
@@ -1123,6 +1133,7 @@ static int bpr_epoch_deterministic(const BprParams& p, int64_t n_users, cudaStre
     B200_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), bytes, st));
     DetState d;
     d.d_max = det_delta_bound(round);
+    d.cap = (unsigned)cap;
     d.acc = reinterpret_cast<unsigned long long*>(buf + rec_b);
     d.n_shared = reinterpret_cast<unsigned int*>(buf + rec_b + acc_b);
     unsigned int* cnt = d.n_shared + n_rounds;
