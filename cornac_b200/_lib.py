@@ -96,6 +96,10 @@ SIGNATURES = {
     "b200_mter_fit": (_int, [_i64] * 4 + [_int] * 4 + ([_vp] * 4 + [_i64]) * 3 + [_vp] * 4 + [_i64] + [_int] * 3 +
                       [_vp] * 4 + [_f32] * 3 + [_int, _u64, _u64] + [_vp] * 4),
     "b200_mter_queries": (_int, [_vp, _i64, _vp, _vp, _int, _int, _int, _vp, _vp]),
+    "b200_comparer_sub_workspace_bytes": (_i64, [_i64] * 4 + [_int] * 7),
+    "b200_comparer_sub_fit": (_int, [_i64] * 4 + [_int] * 4 + ([_vp] * 4 + [_i64]) * 3 + [_vp] * 4 + [_i64] +
+                              [_vp] * 4 + [_i64] + [_int] * 4 + [_vp] * 4 + [_f32] * 4 + [_int, _u64, _u64] + [_vp] * 4),
+    "b200_comparer_rank_rows": (_int, [_vp] * 5 + [_i64, _i64] + [_int] * 3 + [_i64, _int, _c.c_double, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),

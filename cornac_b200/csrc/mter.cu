@@ -1,14 +1,17 @@
-// MTER (cornac/models/mter/recom_mter.pyx:434-675) for sm_90a: the seeded fit, bit-identical to the reference's serial
-// float loop given the same sample draws, and the rank queries of the device scoring path.
+// MTER (cornac/models/mter/recom_mter.pyx:434-675) and ComparERSub (cornac/models/comparer/recom_comparer_sub.pyx:487-760)
+// for sm_90a: the seeded fit, bit-identical to the reference's serial float loop given the same sample draws, the rank
+// queries of MTER's device scoring path and ComparERSub's aspect-mixed score rows.
 //
 // One iteration of the reference reads the parameters it started with everywhere and writes them only in its final
 // AdaGrad step, so it splits into independent chains:
 //   phase 1  the predictions: one f32 chain of d1*d2*d3 terms per element sample, two per BPR sample (the two lanes of
-//            a pair compute score(i) and score(j) side by side and swap them); the sample's coefficient
-//            (2 (pred - score), or lambda_bpr z s) and the ids it touches.
+//            a pair compute score(i) and score(j) side by side and swap them), and ComparERSub's pair samples the
+//            same way (score(later, a) and score(earlier, a)); the sample's coefficient (2 (pred - score), lambda_bpr z s
+//            or lambda_d z) and the ids it touches.  MTER is ComparERSub with no pair samples.
 //   phase 2  which (matrix, row) each touch slot is the first to name: that slot owns the row's accumulator.
 //   phase 3  every accumulator element as one ordered f32 chain over the samples that touch it, in the reference's
-//            order (element samples: uia, uao, iao terms; then the BPR samples; (i, j, k) order inside a sample): a
+//            order (element samples: uia, uao, iao terms; then the BPR samples; then the pair samples; (i, j, k) order
+//            inside a sample): a
 //            thread per core-tensor element and per (owned row, column).  The result goes to a dense `del` buffer.
 //   phase 4  the dense AdaGrad step over every parameter, which also clears `del` for the next iteration.
 // The phases are separated by grid-wide barriers of one cooperative launch, so a call of n iterations is one launch.
@@ -39,20 +42,24 @@ struct MterArgs {
     const int32_t *YI_i, *YI_a, *YI_o;
     const int32_t *indptr, *indices, *rrow;
     const float* rval;
-    int n_el, n_bpr, n_iter;
+    const int32_t *p_u, *p_e, *p_l, *p_a;   // ComparERSub's pair list (user, earlier, later, aspect)
+    int64_t n_plist;
+    int n_el, n_bpr, n_pair, n_iter;
     const int32_t* draws;
     float* P[M_N];
     float* S[M_N];
     float* D[M_N];
     int64_t cnt[M_N];
-    float* coef;       // [3 n_el + n_bpr]: 2 (pred - score) of each element sample, then del_bpr of each BPR sample
-    int32_t* ids;      // [9 n_el + 4 n_bpr]: (u, i, a), (u, a, o), (i, a, o) per element sample, (u, i, j, live) per BPR
-    int64_t* keys;     // [9 n_el + 4 n_bpr]: matrix << 40 | row of every touch slot
-    uint8_t* owner;    // [9 n_el + 4 n_bpr]
-    float lr, ld_reg, ld_bpr;
+    float* coef;       // [3 n_el + n_bpr + n_pair]: 2 (pred - score) of each element sample, del_bpr of each BPR
+                       // sample, del_aspect_bpr of each pair sample
+    int32_t* ids;      // [n_slots]: (u, i, a), (u, a, o), (i, a, o) per element sample, (u, i, j, live) per BPR sample,
+                       // (u, later, earlier, a) per pair sample
+    int64_t* keys;     // [n_slots]: matrix << 40 | row of every touch slot
+    uint8_t* owner;    // [n_slots]
+    float lr, ld_reg, ld_bpr, ld_d;
     int core_smem;
-    unsigned long long* counts;   // += correct, skipped
-    double* losses;               // += loss, bpr_loss (f64)
+    unsigned long long* counts;   // += correct, skipped (and, with pair samples, aspect_correct)
+    double* losses;               // += loss, bpr_loss (and, with pair samples, aspect_bpr_loss) (f64)
     int32_t* first;               // per (matrix, row): n_slots - (first slot naming it), 0 when unnamed
     int64_t row_off[4];           // offset of U, I, A, O rows in `first`
     float* aterms;                // [d3][aterm_stride]: the BPR terms of the A[n_aspects] chain, in chain order
@@ -63,6 +70,12 @@ struct MterArgs {
     int64_t n_x, n_yu, n_yi, nnz;
     unsigned long long* phase_ns; // += device time of each phase (block 0's view), or NULL
 };
+
+// touch slots: 9 per element sample, 4 per BPR sample, 4 per pair sample
+__device__ __forceinline__ int64_t n_slots_of(const MterArgs& a)
+{
+    return 9ll * a.n_el + 4ll * a.n_bpr + 4ll * a.n_pair;
+}
 
 __device__ __forceinline__ float mul4(float a, float b, float c, float d)
 {
@@ -117,12 +130,13 @@ __device__ __forceinline__ int mat_cols(const MterArgs& a, int m)
 __device__ void mter_predict(const MterArgs& a, const int32_t* dr, int it, const float* G1, const float* G2,
                              const float* G3)
 {
-    const int64_t n_slots = 9ll * a.n_el + 4ll * a.n_bpr;
-    const int n_el = a.n_el, n_bpr = a.n_bpr;
+    const int64_t n_slots = n_slots_of(a);
+    const int n_el = a.n_el, n_bpr = a.n_bpr, n_pair = a.n_pair;
     const int d1 = a.d1, d2 = a.d2, d3 = a.d3, d4 = a.d4;
     const float *U = a.P[M_U], *I = a.P[M_I], *A = a.P[M_A], *O = a.P[M_O];
     const float* An = A + a.n_aspects * d3;
-    const int64_t total = 2ll * n_bpr + 3ll * n_el;
+    // work items: two lanes per BPR sample, two per pair sample (both start at an even index), one per element sample
+    const int64_t total = 2ll * n_bpr + 2ll * n_pair + 3ll * n_el;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     int64_t* keys_bpr = a.keys + 9ll * n_el;
     for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total; w += stride) {
@@ -164,8 +178,33 @@ __device__ void mter_predict(const MterArgs& a, const int32_t* dr, int it, const
                     if (a.losses) atomicAdd(a.losses + 1, log(1.0 / (1.0 + (double)glibc_expf(-pred))));
                 }
             }
+        } else if (w < 2ll * n_bpr + 2ll * n_pair) {
+            // pair sample: pred = score(u, later, a) - score(u, earlier, a); lane 0 scores the later item
+            const int t = (int)((w - 2ll * n_bpr) >> 1), side = (int)(w & 1);
+            const int64_t idx = mter_draw(a, dr, it, 3ll * n_el + 2ll * n_bpr + t, a.n_plist);
+            const int32_t u = a.p_u[idx], e = a.p_e[idx], l = a.p_l[idx], as = a.p_a[idx];
+            const float sc = score3(G1, d1, d2, d3, U + (int64_t)u * d1, I + (int64_t)(side ? e : l) * d2, A + (int64_t)as * d3);
+            const unsigned pair = 3u << (threadIdx.x & 30);
+            const float other = __shfl_xor_sync(pair, sc, 1);
+            if (side == 0) {
+                const int64_t s0 = 9ll * n_el + 4ll * n_bpr + 4ll * t;
+                int32_t* id = a.ids + s0;
+                id[0] = u; id[1] = l; id[2] = e; id[3] = as;
+                int64_t* k = a.keys + s0;
+                k[0] = ((int64_t)M_U << 40) | u;
+                k[1] = ((int64_t)M_I << 40) | l;
+                k[2] = ((int64_t)M_I << 40) | e;
+                k[3] = ((int64_t)M_A << 40) | as;
+                if (!a.unordered)
+                    for (int q = 0; q < 4; ++q) atomicMax(a.first + key_index(a, k[q]), (int32_t)(n_slots - (s0 + q)));
+                const float pred = __fsub_rn(sc, other);
+                const float z = __double2float_rn(__ddiv_rn(1.0, __dadd_rn(1.0, (double)glibc_expf(pred))));
+                if ((double)z < 0.5) atomicAdd(a.counts + 2, 1ull);
+                a.coef[3 * n_el + n_bpr + t] = __fmul_rn(a.ld_d, z);
+                if (a.losses) atomicAdd(a.losses + 2, log(1.0 / (1.0 + (double)glibc_expf(-pred))));
+            }
         } else {
-            const int64_t e = w - 2ll * n_bpr;
+            const int64_t e = w - 2ll * n_bpr - 2ll * n_pair;
             const int kind = (int)(e / n_el), t = (int)(e % n_el);
             const int64_t idx = mter_draw(a, dr, it, (int64_t)kind * n_el + t, kind == 0 ? a.n_x : kind == 1 ? a.n_yu : a.n_yi);
             int32_t x, y, zz;
@@ -202,7 +241,7 @@ __device__ void mter_predict(const MterArgs& a, const int32_t* dr, int it, const
 // and every term of the longest chain, A[n_aspects]'s BPR part, stored in chain order so that phase 3 only adds
 __device__ void mter_owners(const MterArgs& a, const float* G1)
 {
-    const int64_t n_slots = 9ll * a.n_el + 4ll * a.n_bpr;
+    const int64_t n_slots = n_slots_of(a);
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     const int64_t gtid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     for (int64_t s = gtid; s < n_slots; s += stride)
@@ -223,6 +262,42 @@ __device__ void mter_owners(const MterArgs& a, const float* G1)
         }
         a.aterms[c * a.aterm_stride + e] = v;
     }
+}
+
+// phase 3, rows: the pair samples' terms of accumulator element (m, row, c), after the BPR samples' (U, I and A rows;
+// a pair's aspect is below n_aspects - 1, so never the stored chain of A[n_aspects])
+__device__ float pair_row_terms(const MterArgs& a, const float* G1, int m, int32_t row, int c, float acc)
+{
+    const int d1 = a.d1, d2 = a.d2, d3 = a.d3;
+    const float *U = a.P[M_U], *I = a.P[M_I], *A = a.P[M_A];
+    const int32_t* ids = a.ids + 9ll * a.n_el + 4ll * a.n_bpr;
+    const float* coef = a.coef + 3 * a.n_el + a.n_bpr;
+    for (int t = 0; t < a.n_pair; ++t) {
+        const int32_t* id = ids + 4ll * t;
+        const int32_t u = id[0], l = id[1], e = id[2], as = id[3];
+        const bool hit = m == M_U ? u == row : m == M_I ? (l == row || e == row) : as == row;
+        if (!hit) continue;
+        const float dp = coef[t];
+        const float *Ur = U + (int64_t)u * d1, *Il = I + (int64_t)l * d2, *Ie = I + (int64_t)e * d2;
+        const float* Ar = A + (int64_t)as * d3;
+        if (m == M_U)
+            for (int q = 0; q < d2; ++q) {
+                const float aji = __fsub_rn(Il[q], Ie[q]);
+                for (int r = 0; r < d3; ++r) acc = __fsub_rn(acc, mul4(dp, G1[(c * d2 + q) * d3 + r], aji, Ar[r]));
+            }
+        else if (m == M_I)            // del_i[later] -= v, then del_i[earlier] += v: both when later == earlier
+            for (int p = 0; p < d1; ++p)
+                for (int r = 0; r < d3; ++r) {
+                    const float v = mul4(dp, G1[(p * d2 + c) * d3 + r], Ur[p], Ar[r]);
+                    if (l == row) acc = __fsub_rn(acc, v);
+                    if (e == row) acc = __fadd_rn(acc, v);
+                }
+        else
+            for (int p = 0; p < d1; ++p)
+                for (int q = 0; q < d2; ++q)
+                    acc = __fsub_rn(acc, mul4(dp, G1[(p * d2 + q) * d3 + c], Ur[p], __fsub_rn(Il[q], Ie[q])));
+    }
+    return acc;
 }
 
 // phase 3, rows: accumulator element (m, row, c) as the reference's loops build it
@@ -281,7 +356,7 @@ __device__ float row_chain(const MterArgs& a, const float* G1, const float* G2, 
     }
     if (m == M_O) return acc;
     if (m == M_A) {
-        if (row != a.n_aspects) return acc;
+        if (row != a.n_aspects) return pair_row_terms(a, G1, m, row, c, acc);
         // the stored terms of phase 2, subtracted in order: only the adds are serial here
         const float* tp = a.aterms + (int64_t)c * a.aterm_stride;
         const int64_t n = (int64_t)n_bpr * d1 * d2, n4 = n / 4;
@@ -323,7 +398,7 @@ __device__ float row_chain(const MterArgs& a, const float* G1, const float* G2, 
                 }
         }
     }
-    return acc;
+    return pair_row_terms(a, G1, m, row, c, acc);
 }
 
 // phase 3, cores: element e of G1, G2 or G3
@@ -347,6 +422,12 @@ __device__ float core_chain(const MterArgs& a, int g, int e)
             const float iij = __fsub_rn(I[(int64_t)id[1] * d2 + q], I[(int64_t)id[2] * d2 + q]);
             acc = __fsub_rn(acc, mul4(a.coef[3 * n_el + t], U[(int64_t)id[0] * d1 + p], iij, an));
         }
+        for (int t = 0; t < a.n_pair; ++t) {
+            const int32_t* id = a.ids + 9ll * n_el + 4ll * n_bpr + 4ll * t;
+            const float aji = __fsub_rn(I[(int64_t)id[1] * d2 + q], I[(int64_t)id[2] * d2 + q]);
+            acc = __fsub_rn(acc, mul4(a.coef[3 * n_el + n_bpr + t], U[(int64_t)id[0] * d1 + p], aji,
+                                      A[(int64_t)id[3] * d3 + r]));
+        }
     } else if (g == 1) {
         const int p = e / (d3 * d4), q = (e / d4) % d3, r = e % d4;
         for (int t = 0; t < n_el; ++t) {
@@ -369,13 +450,14 @@ __device__ void mter_gradients(const MterArgs& a, const float* G1, const float* 
 {
     const int64_t nG1 = a.cnt[M_G1], nG2 = a.cnt[M_G2], nG3 = a.cnt[M_G3];
     const int dmax = max(max(a.d1, a.d2), max(a.d3, a.d4));
-    const int64_t n_slots = 9ll * a.n_el + 4ll * a.n_bpr;
+    const int64_t n_slots = n_slots_of(a);
     const int64_t n_row_items = n_slots * dmax;
     const int64_t total = n_row_items + nG1 + nG2 + nG3;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total; w += stride) {
         if (w < n_row_items) {
-            // the BPR slots (and so the aspect row every BPR sample touches, the longest chain) come first
+            // the BPR slots (and so the aspect row every BPR sample touches, the longest chain) come first, then the
+            // pair slots
             const int64_t s = (w / dmax + 9ll * a.n_el) % n_slots;
             const int c = (int)(w % dmax);
             if (!a.owner[s]) continue;
@@ -422,7 +504,8 @@ __device__ void mter_adagrad(const MterArgs& a)
 // Unordered mode, phase 3: the core elements as in the exact mode (each a short chain over the samples), and one warp
 // per sample adding its row gradients with atomics: for a sample (x, y, w) of core G and weight c,
 // dx[p] += c sum_qr G[p,q,r] y[q] w[r], dy[q] += c sum_pr G[p,q,r] x[p] w[r], dw[r] += c sum_pq G[p,q,r] x[p] y[q]
-// (a BPR sample: x = U[u], y = I[i] - I[j], w = A[n_aspects], c = -del_bpr, and I[j] takes -dy).  f32 atomics: the
+// (a BPR sample: x = U[u], y = I[i] - I[j], w = A[n_aspects], c = -del_bpr, and I[j] takes -dy; a pair sample:
+// x = U[u], y = I[later] - I[earlier], w = A[a], c = -del_aspect_bpr, and I[earlier] takes -dy).  f32 atomics: the
 // sums are not in a fixed order, so the result can differ from run to run by rounding.
 __device__ void sample_rows(const float* G, int n1, int n2, int n3, const float* x, const float* y, const float* y2,
                             const float* w, float c, float* dx, float* dy, float* dy2, float* dw, int lane)
@@ -466,7 +549,7 @@ __device__ void mter_gradients_unordered(const MterArgs& a, const float* G1, con
     const float *U = a.P[M_U], *I = a.P[M_I], *A = a.P[M_A], *O = a.P[M_O];
     float *dU = a.D[M_U], *dI = a.D[M_I], *dA = a.D[M_A], *dO = a.D[M_O];
     const int lane = threadIdx.x & 31;
-    const int64_t n_samples = 3ll * n_el + a.n_bpr;
+    const int64_t n_samples = 3ll * n_el + a.n_bpr + a.n_pair;
     for (int64_t sm = gtid >> 5; sm < n_samples; sm += stride >> 5) {
         const float c = a.coef[sm];
         if (sm < 3ll * n_el) {
@@ -484,12 +567,17 @@ __device__ void mter_gradients_unordered(const MterArgs& a, const float* G1, con
                 sample_rows(G3, d2, d3, d4, I + (int64_t)id[0] * d2, A + (int64_t)id[1] * d3, nullptr,
                             O + (int64_t)id[2] * d4, c, dI + (int64_t)id[0] * d2, dA + (int64_t)id[1] * d3, nullptr,
                             dO + (int64_t)id[2] * d4, lane);
-        } else {
+        } else if (sm < 3ll * n_el + a.n_bpr) {
             const int32_t* id = a.ids + 9ll * n_el + 4ll * (sm - 3ll * n_el);
             if (!id[3]) continue;
             sample_rows(G1, d1, d2, d3, U + (int64_t)id[0] * d1, I + (int64_t)id[1] * d2, I + (int64_t)id[2] * d2,
                         A + a.n_aspects * d3, -c, dU + (int64_t)id[0] * d1, dI + (int64_t)id[1] * d2,
                         dI + (int64_t)id[2] * d2, dA + a.n_aspects * d3, lane);
+        } else {
+            const int32_t* id = a.ids + 9ll * n_el + 4ll * a.n_bpr + 4ll * (sm - 3ll * n_el - a.n_bpr);
+            sample_rows(G1, d1, d2, d3, U + (int64_t)id[0] * d1, I + (int64_t)id[1] * d2, I + (int64_t)id[2] * d2,
+                        A + (int64_t)id[3] * d3, -c, dU + (int64_t)id[0] * d1, dI + (int64_t)id[1] * d2,
+                        dI + (int64_t)id[2] * d2, dA + (int64_t)id[3] * d3, lane);
         }
     }
 }
@@ -505,7 +593,7 @@ __global__ void __launch_bounds__(MTER_THREADS) mter_fit_kernel(MterArgs a)
 {
     extern __shared__ float sh_core[];
     cg::grid_group grid = cg::this_grid();
-    const int64_t per_iter = 3ll * a.n_el + 2ll * a.n_bpr;
+    const int64_t per_iter = 3ll * a.n_el + 2ll * a.n_bpr + a.n_pair;
     const int64_t nG1 = a.cnt[M_G1], nG2 = a.cnt[M_G2], nG3 = a.cnt[M_G3];
     const float *G1 = a.P[M_G1], *G2 = a.P[M_G2], *G3 = a.P[M_G3];
     if (a.core_smem) {
@@ -570,6 +658,104 @@ __global__ void __launch_bounds__(MTER_THREADS) mter_queries_kernel(const float*
     }
 }
 
+// ComparERSub's rank rows (recom_comparer_sub.pyx:762-806), all in f64 and rounded once to f32: for user u,
+//   B[q, r] = sum_p G1[p, q, r] U[u, p],   P[q, a] = sum_r B[q, r] A[a, r]   (a <= n_aspects; kept in f64)
+//   ts3[i, a] = sum_q I[i, q] P[q, a]
+//   score[i] = f32(alpha * (sum of the n_top largest ts3[i, a < n_aspects]) / n_top + (1 - alpha) * ts3[i, n_aspects])
+// every sum in index order.  A block per (user, tile of CR_ITEMS items) builds B and P in shared memory; a warp per item
+// holds ts3[i, lane + 32 j] in registers.  The n_top-th largest value is found exactly by bisection over the 64 bits of
+// an order-preserving integer key (the largest key k with at least n_top keys >= k); the sum of the top n_top is then
+// the values above it plus (n_top - their count) copies of it, which is well defined at ties.
+constexpr int CR_THREADS = 256, CR_ITEMS = 64;
+
+__device__ __forceinline__ uint64_t f64_key(double v)
+{
+    const uint64_t b = (uint64_t)__double_as_longlong(v);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+__device__ __forceinline__ double key_f64(uint64_t k)
+{
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+template <int J>
+__global__ void __launch_bounds__(CR_THREADS) comparer_rank_kernel(const float* __restrict__ U,
+                                                                   const float* __restrict__ I,
+                                                                   const float* __restrict__ A,
+                                                                   const float* __restrict__ G1,
+                                                                   const int64_t* __restrict__ users, int64_t n_items,
+                                                                   int d1, int d2, int d3, int n_aspects, int n_top,
+                                                                   double alpha, double beta, float* __restrict__ out)
+{
+    extern __shared__ double sh_p[];
+    const int na1 = n_aspects + 1;
+    double* B = sh_p;                       // [d2][d3]
+    double* P = sh_p + d2 * d3;             // [d2][n_aspects + 1]
+    const int64_t u = users[blockIdx.y];
+    const float* Uu = U + u * d1;
+    for (int e = threadIdx.x; e < d2 * d3; e += blockDim.x) {
+        double s = 0.0;
+        for (int p = 0; p < d1; ++p) s = __dadd_rn(s, __dmul_rn((double)G1[(int64_t)p * d2 * d3 + e], (double)Uu[p]));
+        B[e] = s;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < d2 * na1; e += blockDim.x) {
+        const int q = e / na1, as = e % na1;
+        double s = 0.0;
+        for (int r = 0; r < d3; ++r) s = __dadd_rn(s, __dmul_rn(B[q * d3 + r], (double)A[(int64_t)as * d3 + r]));
+        P[e] = s;
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int64_t i1 = min(n_items, (int64_t)(blockIdx.x + 1) * CR_ITEMS);
+    for (int64_t i = (int64_t)blockIdx.x * CR_ITEMS + (threadIdx.x >> 5); i < i1; i += CR_THREADS / 32) {
+        const float* Ii = I + i * d2;
+        double v[J];
+#pragma unroll
+        for (int j = 0; j < J; ++j) v[j] = 0.0;
+        for (int q = 0; q < d2; ++q) {
+            const double iq = (double)Ii[q];
+#pragma unroll
+            for (int j = 0; j < J; ++j)
+                if (lane + 32 * j < na1) v[j] = __dadd_rn(v[j], __dmul_rn(iq, P[q * na1 + lane + 32 * j]));
+        }
+        double last = 0.0;
+        uint64_t key[J];                    // 0 (below every value's key) outside the aspects
+#pragma unroll
+        for (int j = 0; j < J; ++j) {
+            const int as = lane + 32 * j;
+            if (as == n_aspects) last = v[j];
+            key[j] = as < n_aspects ? f64_key(v[j]) : 0ull;
+        }
+        last = __shfl_sync(0xffffffffu, last, n_aspects & 31);
+        uint64_t kth = 0;                   // the key of the n_top-th largest value; 0: every value is taken
+        if (n_top < n_aspects)
+            for (int bit = 63; bit >= 0; --bit) {
+                const uint64_t cand = kth | (1ull << bit);
+                int c = 0;
+#pragma unroll
+                for (int j = 0; j < J; ++j) c += key[j] >= cand;
+                if (__reduce_add_sync(0xffffffffu, c) >= n_top) kth = cand;
+            }
+        double s = 0.0;
+        int above = 0;
+#pragma unroll
+        for (int j = 0; j < J; ++j)
+            if (key[j] > kth) {
+                s = __dadd_rn(s, v[j]);
+                ++above;
+            }
+        for (int off = 16; off > 0; off >>= 1) s = __dadd_rn(s, __shfl_xor_sync(0xffffffffu, s, off));
+        above = __reduce_add_sync(0xffffffffu, above);
+        if (lane == 0) {
+            if (above < n_top) s = __dadd_rn(s, __dmul_rn((double)(n_top - above), key_f64(kth)));
+            const double mean = __ddiv_rn(s, (double)n_top);
+            out[(int64_t)blockIdx.y * n_items + i] = __double2float_rn(__dadd_rn(__dmul_rn(alpha, mean), __dmul_rn(beta, last)));
+        }
+    }
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -596,11 +782,11 @@ struct MterLayout {
 };
 
 static MterLayout mter_layout(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1, int d2,
-                              int d3, int d4, int n_el, int n_bpr)
+                              int d3, int d4, int n_el, int n_bpr, int n_pair)
 {
     int64_t cnt[M_N];
     const int64_t params = mter_counts(n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, cnt);
-    const int64_t slots = 9ll * n_el + 4ll * n_bpr;
+    const int64_t slots = 9ll * n_el + 4ll * n_bpr + 4ll * n_pair;
     auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
     MterLayout l{};
     l.rows = n_users + n_items + n_aspects + 1 + n_opinions;
@@ -608,7 +794,7 @@ static MterLayout mter_layout(int64_t n_users, int64_t n_items, int64_t n_aspect
     l.del = 0;
     l.first = l.del + up(4 * params);
     l.coef = l.first + up(4 * l.rows);
-    l.ids = l.coef + up(4 * (3ll * n_el + n_bpr));
+    l.ids = l.coef + up(4 * (3ll * n_el + n_bpr + n_pair));
     l.keys = l.ids + up(4 * slots);
     l.owner = l.keys + up(8 * slots);
     l.aterms = l.owner + up(slots);
@@ -619,36 +805,50 @@ static MterLayout mter_layout(int64_t n_users, int64_t n_items, int64_t n_aspect
 extern "C" int64_t b200_mter_workspace_bytes(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions,
                                              int d1, int d2, int d3, int d4, int n_el, int n_bpr)
 {
-    return mter_layout(n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, n_el, n_bpr).total;
+    return mter_layout(n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, n_el, n_bpr, 0).total;
 }
 
-extern "C" int b200_mter_fit(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1, int d2,
-                             int d3, int d4, const float* X, const int32_t* X_u, const int32_t* X_i, const int32_t* X_a,
-                             int64_t n_x, const float* YU, const int32_t* YU_u, const int32_t* YU_a,
-                             const int32_t* YU_o, int64_t n_yu, const float* YI, const int32_t* YI_i,
-                             const int32_t* YI_a, const int32_t* YI_o, int64_t n_yi, const int32_t* indptr,
-                             const int32_t* indices, const int32_t* rrow, const float* rval, int64_t nnz, int n_el,
-                             int n_bpr, int n_iter, const int32_t* draws, float* const* params, float* const* sgrad,
-                             void* work, float lr, float lambda_reg, float lambda_bpr, int flags, uint64_t seed,
-                             uint64_t iter0, unsigned long long* counts, double* losses, unsigned long long* phase_ns,
-                             void* stream)
+extern "C" int64_t b200_comparer_sub_workspace_bytes(int64_t n_users, int64_t n_items, int64_t n_aspects,
+                                                     int64_t n_opinions, int d1, int d2, int d3, int d4, int n_el,
+                                                     int n_bpr, int n_pair)
+{
+    return mter_layout(n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, n_el, n_bpr, n_pair).total;
+}
+
+// The fit of both models: MTER is the case n_pair = 0 (no pair list, no pair samples).
+static int mter_launch(const char* fn, int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1,
+                       int d2, int d3, int d4, const float* X, const int32_t* X_u, const int32_t* X_i,
+                       const int32_t* X_a, int64_t n_x, const float* YU, const int32_t* YU_u, const int32_t* YU_a,
+                       const int32_t* YU_o, int64_t n_yu, const float* YI, const int32_t* YI_i, const int32_t* YI_a,
+                       const int32_t* YI_o, int64_t n_yi, const int32_t* indptr, const int32_t* indices,
+                       const int32_t* rrow, const float* rval, int64_t nnz, const int32_t* p_u, const int32_t* p_e,
+                       const int32_t* p_l, const int32_t* p_a, int64_t n_plist, int n_el, int n_bpr, int n_pair,
+                       int n_iter, const int32_t* draws, float* const* params, float* const* sgrad, void* work,
+                       float lr, float lambda_reg, float lambda_bpr, float lambda_d, int flags, uint64_t seed,
+                       uint64_t iter0, unsigned long long* counts, double* losses, unsigned long long* phase_ns,
+                       void* stream)
 {
     B200_REQUIRE(n_users > 0 && n_items > 0 && n_aspects >= 0 && n_opinions > 0 && d1 > 0 && d2 > 0 && d3 > 0 &&
                      d4 > 0 && n_el > 0 && n_bpr > 0 && n_iter >= 0 && nnz > 0 && n_x > 0 && n_yu > 0 && n_yi > 0,
-                 "b200_mter_fit: bad sizes (users %lld items %lld aspects %lld opinions %lld factors %d/%d/%d/%d "
-                 "samples %d/%d iterations %d ratings %lld tensors %lld/%lld/%lld)",
+                 "%s: bad sizes (users %lld items %lld aspects %lld opinions %lld factors %d/%d/%d/%d "
+                 "samples %d/%d iterations %d ratings %lld tensors %lld/%lld/%lld)", fn,
                  (long long)n_users, (long long)n_items, (long long)n_aspects, (long long)n_opinions, d1, d2, d3, d4,
                  n_el, n_bpr, n_iter, (long long)nnz, (long long)n_x, (long long)n_yu, (long long)n_yi);
+    B200_REQUIRE(n_pair >= 0 && n_plist >= 0 && (n_pair == 0 || n_plist > 0),
+                 "%s: %d pair samples from a pair list of %lld", fn, n_pair, (long long)n_plist);
     B200_REQUIRE(n_aspects + 1 < (1ll << 31) && n_users < (1ll << 31) && n_items < (1ll << 31) &&
-                     n_opinions < (1ll << 31) && nnz < (1ll << 31) && 9ll * n_el + 4ll * n_bpr < (1ll << 31),
-                 "b200_mter_fit: sizes beyond int32 ids");
+                     n_opinions < (1ll << 31) && nnz < (1ll << 31) &&
+                     9ll * n_el + 4ll * n_bpr + 4ll * n_pair < (1ll << 31),
+                 "%s: sizes beyond int32 ids", fn);
     B200_REQUIRE(X && X_u && X_i && X_a && YU && YU_u && YU_a && YU_o && YI && YI_i && YI_a && YI_o && indptr &&
-                     indices && rrow && rval && params && sgrad && work && counts,
-                 "b200_mter_fit: null pointer argument");
-    B200_REQUIRE((flags & ~(B200_MTER_UNORDERED | B200_MTER_PHILOX)) == 0, "b200_mter_fit: unknown flags %d", flags);
+                     indices && rrow && rval && params && sgrad && work && counts &&
+                     (n_pair == 0 || (p_u && p_e && p_l && p_a)),
+                 "%s: null pointer argument", fn);
+    B200_REQUIRE((flags & ~(B200_MTER_UNORDERED | B200_MTER_PHILOX)) == 0, "%s: unknown flags %d", fn, flags);
     if (n_iter == 0) return B200_OK;
-    B200_REQUIRE(draws || (flags & B200_MTER_PHILOX), "b200_mter_fit: null draws");
+    B200_REQUIRE(draws || (flags & B200_MTER_PHILOX), "%s: null draws", fn);
     MterArgs a{};
+    a.p_u = p_u; a.p_e = p_e; a.p_l = p_l; a.p_a = p_a; a.n_plist = n_plist; a.n_pair = n_pair; a.ld_d = lambda_d;
     a.n_users = n_users; a.n_items = n_items; a.n_aspects = n_aspects; a.n_opinions = n_opinions;
     a.d1 = d1; a.d2 = d2; a.d3 = d3; a.d4 = d4;
     a.X = X; a.X_u = X_u; a.X_i = X_i; a.X_a = X_a;
@@ -660,9 +860,9 @@ extern "C" int b200_mter_fit(int64_t n_users, int64_t n_items, int64_t n_aspects
     for (int m = 0; m < M_N; ++m) {
         a.P[m] = params[m];
         a.S[m] = sgrad[m];
-        B200_REQUIRE(a.P[m] && a.S[m], "b200_mter_fit: null parameter or AdaGrad state %d", m);
+        B200_REQUIRE(a.P[m] && a.S[m], "%s: null parameter or AdaGrad state %d", fn, m);
     }
-    const MterLayout l = mter_layout(n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, n_el, n_bpr);
+    const MterLayout l = mter_layout(n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, n_el, n_bpr, n_pair);
     char* w = (char*)work;
     float* del = (float*)(w + l.del);
     for (int m = 0; m < M_N; ++m) {
@@ -700,13 +900,51 @@ extern "C" int b200_mter_fit(int64_t n_users, int64_t n_items, int64_t n_aspects
     B200_CUDA(cudaFuncSetAttribute(mter_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
     B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mter_fit_kernel, MTER_THREADS, smem));
-    B200_REQUIRE(per_sm > 0, "b200_mter_fit: the fit kernel does not fit on an SM");
+    B200_REQUIRE(per_sm > 0, "%s: the fit kernel does not fit on an SM", fn);
     const int blocks = sm_count() * per_sm;
     void* kargs[] = {&a};
     count_launch();
     B200_CUDA(cudaLaunchCooperativeKernel((const void*)mter_fit_kernel, dim3(blocks), dim3(MTER_THREADS), kargs, smem,
                                           (cudaStream_t)stream));
     return B200_OK;
+}
+
+extern "C" int b200_mter_fit(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1, int d2,
+                             int d3, int d4, const float* X, const int32_t* X_u, const int32_t* X_i, const int32_t* X_a,
+                             int64_t n_x, const float* YU, const int32_t* YU_u, const int32_t* YU_a,
+                             const int32_t* YU_o, int64_t n_yu, const float* YI, const int32_t* YI_i,
+                             const int32_t* YI_a, const int32_t* YI_o, int64_t n_yi, const int32_t* indptr,
+                             const int32_t* indices, const int32_t* rrow, const float* rval, int64_t nnz, int n_el,
+                             int n_bpr, int n_iter, const int32_t* draws, float* const* params, float* const* sgrad,
+                             void* work, float lr, float lambda_reg, float lambda_bpr, int flags, uint64_t seed,
+                             uint64_t iter0, unsigned long long* counts, double* losses, unsigned long long* phase_ns,
+                             void* stream)
+{
+    return mter_launch("b200_mter_fit", n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, X, X_u, X_i, X_a, n_x,
+                       YU, YU_u, YU_a, YU_o, n_yu, YI, YI_i, YI_a, YI_o, n_yi, indptr, indices, rrow, rval, nnz,
+                       nullptr, nullptr, nullptr, nullptr, 0, n_el, n_bpr, 0, n_iter, draws, params, sgrad, work, lr,
+                       lambda_reg, lambda_bpr, 0.f, flags, seed, iter0, counts, losses, phase_ns, stream);
+}
+
+extern "C" int b200_comparer_sub_fit(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1,
+                                     int d2, int d3, int d4, const float* X, const int32_t* X_u, const int32_t* X_i,
+                                     const int32_t* X_a, int64_t n_x, const float* YU, const int32_t* YU_u,
+                                     const int32_t* YU_a, const int32_t* YU_o, int64_t n_yu, const float* YI,
+                                     const int32_t* YI_i, const int32_t* YI_a, const int32_t* YI_o, int64_t n_yi,
+                                     const int32_t* indptr, const int32_t* indices, const int32_t* rrow,
+                                     const float* rval, int64_t nnz, const int32_t* p_user, const int32_t* p_earlier,
+                                     const int32_t* p_later, const int32_t* p_aspect, int64_t n_plist, int n_el,
+                                     int n_bpr, int n_pair, int n_iter, const int32_t* draws, float* const* params,
+                                     float* const* sgrad, void* work, float lr, float lambda_reg, float lambda_bpr,
+                                     float lambda_d, int flags, uint64_t seed, uint64_t iter0,
+                                     unsigned long long* counts, double* losses, unsigned long long* phase_ns,
+                                     void* stream)
+{
+    return mter_launch("b200_comparer_sub_fit", n_users, n_items, n_aspects, n_opinions, d1, d2, d3, d4, X, X_u, X_i,
+                       X_a, n_x, YU, YU_u, YU_a, YU_o, n_yu, YI, YI_i, YI_a, YI_o, n_yi, indptr, indices, rrow, rval,
+                       nnz, p_user, p_earlier, p_later, p_aspect, n_plist, n_el, n_bpr, n_pair, n_iter, draws, params,
+                       sgrad, work, lr, lambda_reg, lambda_bpr, lambda_d, flags, seed, iter0, counts, losses, phase_ns,
+                       stream);
 }
 
 extern "C" int b200_mter_queries(const float* U, int64_t n_users, const float* G1, const float* a_last, int d1, int d2,
@@ -723,4 +961,39 @@ extern "C" int b200_mter_queries(const float* U, int64_t n_users, const float* G
                                                                                              d2, d3, Q);
     B200_CUDA(cudaGetLastError());
     return B200_OK;
+}
+
+extern "C" int b200_comparer_rank_rows(const float* U, const float* I, const float* A, const float* G1,
+                                       const int64_t* users, int64_t n_q, int64_t n_items, int d1, int d2, int d3,
+                                       int64_t n_aspects, int n_top, double alpha, float* out, void* stream)
+{
+    B200_REQUIRE(n_q >= 0 && n_items >= 0 && d1 > 0 && d2 > 0 && d3 > 0 && n_aspects > 0 && n_aspects < 1024 &&
+                     n_top > 0 && n_top <= n_aspects,
+                 "b200_comparer_rank_rows: bad sizes n_q=%lld n_items=%lld d=%d/%d/%d aspects=%lld top=%d",
+                 (long long)n_q, (long long)n_items, d1, d2, d3, (long long)n_aspects, n_top);
+    B200_REQUIRE(U && I && A && G1 && users && out, "b200_comparer_rank_rows: null pointer argument");
+    const size_t smem = 8 * ((size_t)d2 * d3 + (size_t)d2 * (n_aspects + 1));
+    B200_REQUIRE(smem <= 200 * 1024, "b200_comparer_rank_rows: %d item factors x %lld aspects exceed shared memory", d2,
+                 (long long)n_aspects);
+    if (n_q == 0 || n_items == 0) return B200_OK;
+    const int na1 = (int)n_aspects + 1;
+    auto launch = [&](auto kernel) -> int {
+        B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const int64_t tiles = (n_items + CR_ITEMS - 1) / CR_ITEMS;
+        for (int64_t q0 = 0; q0 < n_q; q0 += 65535) {
+            const int64_t nq = std::min<int64_t>(65535, n_q - q0);
+            count_launch();
+            kernel<<<dim3((unsigned)tiles, (unsigned)nq), CR_THREADS, smem, (cudaStream_t)stream>>>(
+                U, I, A, G1, users + q0, n_items, d1, d2, d3, (int)n_aspects, n_top, alpha, 1.0 - alpha,
+                out + q0 * n_items);
+            B200_CUDA(cudaGetLastError());
+        }
+        return B200_OK;
+    };
+    if (na1 <= 32) return launch(comparer_rank_kernel<1>);
+    if (na1 <= 64) return launch(comparer_rank_kernel<2>);
+    if (na1 <= 128) return launch(comparer_rank_kernel<4>);
+    if (na1 <= 256) return launch(comparer_rank_kernel<8>);
+    if (na1 <= 512) return launch(comparer_rank_kernel<16>);
+    return launch(comparer_rank_kernel<32>);
 }

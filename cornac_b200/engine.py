@@ -17,6 +17,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     c2pf_fit / c2pf_update  <-> c2pf_cpp / tc2pf_cpp / rc2pf_cpp  (cornac/models/c2pf/cpp/cpp_c2pf.cpp)
     efm_fit / efm_queries   <-> EFM._fit_efm / EFM.rank  (cornac/models/efm/recom_efm.pyx:268-353, 471-528)
     mter_fit / mter_queries <-> MTER._fit_mter / MTER.score (cornac/models/mter/recom_mter.pyx:434-714)
+    comparer_sub_fit / comparer_rank_rows <-> ComparERSub._fit_mter / rank (recom_comparer_sub.pyx:487-806)
 """
 import ctypes
 
@@ -1117,13 +1118,15 @@ class MterData:
 
 class MterDraws:
     """The five seeded sample streams, drawn on the host in chunks of iterations and uploaded through two pinned
-    buffers: chunk k + 1 is drawn while the GPU runs chunk k."""
+    buffers: chunk k + 1 is drawn while the GPU runs chunk k.  `extra`: (seed, hi, n) of further streams, whose n draws
+    of an iteration follow the five's."""
 
-    def __init__(self, seeds, data, n_el, n_bpr, max_chunk):
-        self.samplers = [MTSampler(s) for s in seeds]
+    def __init__(self, seeds, data, n_el, n_bpr, max_chunk, extra=()):
+        self.samplers = [MTSampler(s) for s in seeds] + [MTSampler(s) for s, _, _ in extra]
         self.hi = [len(data.X) - 1, len(data.YU) - 1, len(data.YI) - 1, len(data.indices) - 1, data.n_items - 1]
-        self.n = [n_el, n_el, n_el, n_bpr, n_bpr]
-        self.per_iter = 3 * n_el + 2 * n_bpr
+        self.hi += [int(hi) for _, hi, _ in extra]
+        self.n = [n_el, n_el, n_el, n_bpr, n_bpr] + [int(n) for _, _, n in extra]
+        self.per_iter = sum(self.n)
         self.chunk = max(1, min(int(max_chunk), _MTER_DRAW_CHUNK // self.per_iter))
         self.host = [torch.empty((self.chunk, self.per_iter), dtype=torch.int32).pin_memory() for _ in range(2)]
         self.dev = [torch.empty((self.chunk, self.per_iter), dtype=torch.int32, device="cuda") for _ in range(2)]
@@ -1170,10 +1173,36 @@ class MterDeviceData:
         return [self.n_users, self.n_items, self.n_aspects, self.n_opinions]
 
 
+def comparer_draws(seeds, data, n_el, n_bpr, n_pair, max_chunk):
+    """ComparERSub's six seeded streams as an MterDraws.  `seeds` in the reference's order (uia, uao, iao, pair, pos,
+    neg); an iteration's draws are MTER's five streams', then the n_pair draws of the pair stream over the pair list of
+    `data` (ComparerData).  With n_pair = 0 the pair stream is seeded but never drawn from."""
+    uia, uao, iao, pair, pos, neg = seeds
+    extra = [(pair, len(data.p_user_indices) - 1, n_pair)] if n_pair > 0 else []
+    return MterDraws([uia, uao, iao, pos, neg], data, n_el, n_bpr, max_chunk, extra=extra)
+
+
+class ComparerDeviceData(MterDeviceData):
+    """MterDeviceData plus ComparERSub's pair list (user, earlier, later, aspect), in the reference's order."""
+
+    def __init__(self, data):
+        super().__init__(data)
+        i32 = lambda a: to_device(_pad(np.asarray(a, dtype=np.int32)), torch.int32)      # noqa: E731
+        self.pairs = [i32(data.p_user_indices), i32(data.earlier_indices), i32(data.later_indices),
+                      i32(data.aspect_indices)]
+        self.n_plist = len(data.p_user_indices)
+
+
 def mter_workspace_bytes(data, dims, n_el, n_bpr):
     L_ = require_cuda()
     return int(L_.b200_mter_workspace_bytes(data.n_users, data.n_items, data.n_aspects, data.n_opinions, *dims,
                                             int(n_el), int(n_bpr)))
+
+
+def comparer_sub_workspace_bytes(data, dims, n_el, n_bpr, n_pair):
+    L_ = require_cuda()
+    return int(L_.b200_comparer_sub_workspace_bytes(data.n_users, data.n_items, data.n_aspects, data.n_opinions,
+                                                    *dims, int(n_el), int(n_bpr), int(n_pair)))
 
 
 def mter_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, lr=0.1, lambda_reg=0.1, lambda_bpr=10.0, counts=None,
@@ -1187,7 +1216,30 @@ def mter_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, lr=0.1, lambda_reg
     unordered: sum the rows' gradients per sample with f32 atomics (no fixed order).  philox_seed: draw on the device
     from Philox4x32-10 with this key, iterations iter0, iter0 + 1, ... (draws is then ignored and may be None).
     phase_ns: int64 device [4] or None (+= nanoseconds of the predictions, owners + stored terms, gradients, AdaGrad)."""
+    return _tensor_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, 0, lr, lambda_reg, lambda_bpr, 0.0, counts,
+                       losses, workspace, unordered, philox_seed, iter0, phase_ns)
+
+
+def comparer_sub_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, n_pair, lr=0.5, lambda_reg=0.1, lambda_bpr=10.0,
+                     lambda_d=0.01, counts=None, losses=None, workspace=None, unordered=False, philox_seed=None, iter0=0,
+                     phase_ns=None):
+    """n_iter iterations of ComparERSub._fit_mter (recom_comparer_sub.pyx:487-760) over `data` (ComparerDeviceData):
+    mter_fit plus n_pair samples per iteration from the pair list, bit for bit as the reference's serial f32 loop given
+    the draws.  draws: int32 device tensor [n_iter, 3 n_el + 2 n_bpr + n_pair] (ComparerDraws' layout).  counts: int64
+    device [3] (+= correct, skipped, aspect_correct).  losses: f64 device [3] or None (+= loss, bpr_loss,
+    aspect_bpr_loss).  workspace: of comparer_sub_workspace_bytes.  The other arguments are mter_fit's."""
+    if int(n_pair) < 0 or (int(n_pair) > 0 and data.n_plist == 0):
+        raise B200Error("%d pair samples from a pair list of %d" % (int(n_pair), data.n_plist))
+    return _tensor_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, int(n_pair), lr, lambda_reg, lambda_bpr,
+                       lambda_d, counts, losses, workspace, unordered, philox_seed, iter0, phase_ns)
+
+
+def _tensor_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, n_pair, lr, lambda_reg, lambda_bpr, lambda_d, counts,
+                losses, workspace, unordered, philox_seed, iter0, phase_ns):
+    """mter_fit (n_pair = 0, b200_mter_fit) and comparer_sub_fit (b200_comparer_sub_fit)."""
     L_ = require_cuda()
+    comparer = isinstance(data, ComparerDeviceData)
+    n_counts = 3 if comparer else 2
     U, I, A, O, G1, G2, G3 = params
     dims = (int(G1.shape[0]), int(G1.shape[1]), int(G2.shape[1]), int(G2.shape[2]))
     d1, d2, d3, d4 = dims
@@ -1198,21 +1250,25 @@ def mter_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, lr=0.1, lambda_reg
         if tuple(t.shape) != shape or tuple(st.shape) != shape:
             raise B200Error("%s and its AdaGrad sum must have shape %s, got %s / %s"
                             % (name, shape, tuple(t.shape), tuple(st.shape)))
-    per_iter = 3 * int(n_el) + 2 * int(n_bpr)
+    per_iter = 3 * int(n_el) + 2 * int(n_bpr) + int(n_pair)
     if philox_seed is None:
         _dev(draws, torch.int32, "draws")
         if draws.numel() < int(n_iter) * per_iter:
-            raise B200Error("draws must hold n_iter * (3 n_el + 2 n_bpr) = %d values" % (int(n_iter) * per_iter))
+            raise B200Error("draws must hold n_iter * (3 n_el + 2 n_bpr%s) = %d values"
+                            % (" + n_pair" if comparer else "", int(n_iter) * per_iter))
     else:
         draws = None
     if phase_ns is not None:
         _dev(phase_ns, torch.int64, "phase_ns")
     if counts is None:
-        counts = torch.zeros(2, dtype=torch.int64, device="cuda")
+        counts = torch.zeros(n_counts, dtype=torch.int64, device="cuda")
     _dev(counts, torch.int64, "counts")
     if losses is not None:
         _dev(losses, torch.float64, "losses")
-    need = mter_workspace_bytes(data, dims, n_el, n_bpr)
+    if comparer and (counts.numel() < 3 or (losses is not None and losses.numel() < 3)):
+        raise B200Error("counts and losses must hold 3 values")
+    need = (comparer_sub_workspace_bytes(data, dims, n_el, n_bpr, n_pair) if comparer else
+            mter_workspace_bytes(data, dims, n_el, n_bpr))
     if workspace is None:
         workspace = torch.zeros(need, dtype=torch.uint8, device="cuda")
     _dev(workspace, torch.uint8, "workspace")
@@ -1221,14 +1277,20 @@ def mter_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, lr=0.1, lambda_reg
     pp = (ctypes.c_void_p * 7)(*[ptr(t) for t in params])
     ps = (ctypes.c_void_p * 7)(*[ptr(t) for t in sgrad])
     f32 = lambda x: float(np.float32(x))              # noqa: E731
-    check(L_.b200_mter_fit(*data.args(), *dims, *[ptr(t) for t in data.x], data.n_x, *[ptr(t) for t in data.yu],
-                           data.n_yu, *[ptr(t) for t in data.yi], data.n_yi, *[ptr(t) for t in data.csr], data.nnz,
-                           int(n_el), int(n_bpr), int(n_iter), ptr(draws), pp, ps, ptr(workspace), f32(lr),
-                           f32(lambda_reg), f32(lambda_bpr),
-                           (_lib.MTER_UNORDERED if unordered else 0) | (0 if philox_seed is None else _lib.MTER_PHILOX),
-                           int(philox_seed or 0) & (2 ** 64 - 1), int(iter0), ptr(counts), ptr(losses), ptr(phase_ns),
-                           current_stream()),
-          "b200_mter_fit")
+    head = [*data.args(), *dims, *[ptr(t) for t in data.x], data.n_x, *[ptr(t) for t in data.yu], data.n_yu,
+            *[ptr(t) for t in data.yi], data.n_yi, *[ptr(t) for t in data.csr], data.nnz]
+    flags = (_lib.MTER_UNORDERED if unordered else 0) | (0 if philox_seed is None else _lib.MTER_PHILOX)
+    tail = [flags, int(philox_seed or 0) & (2 ** 64 - 1), int(iter0), ptr(counts), ptr(losses), ptr(phase_ns),
+            current_stream()]
+    if comparer:
+        check(L_.b200_comparer_sub_fit(*head, *[ptr(t) for t in data.pairs], data.n_plist, int(n_el), int(n_bpr),
+                                       int(n_pair), int(n_iter), ptr(draws), pp, ps, ptr(workspace), f32(lr),
+                                       f32(lambda_reg), f32(lambda_bpr), f32(lambda_d), *tail),
+              "b200_comparer_sub_fit")
+    else:
+        check(L_.b200_mter_fit(*head, int(n_el), int(n_bpr), int(n_iter), ptr(draws), pp, ps, ptr(workspace), f32(lr),
+                               f32(lambda_reg), f32(lambda_bpr), *tail),
+              "b200_mter_fit")
     return counts
 
 
@@ -1245,6 +1307,35 @@ def mter_queries(U, G1, A):
     check(L_.b200_mter_queries(ptr(U), int(U.shape[0]), ptr(G1), ptr(A[-1]), d1, d2, d3, ptr(Q), current_stream()),
           "b200_mter_queries")
     return Q
+
+
+def comparer_rank_rows(U, I, A, G1, user_idx, n_top, alpha, n_items=None, out=None):
+    """[n_q, n_items] f32 device rank rows of ComparERSub (b200_comparer_rank_rows): for each user u of user_idx
+    (int64 device) and item i < n_items (default all rows of I), alpha * mean(the n_top largest ts3[i, a < n_aspects])
+    + (1 - alpha) * ts3[i, n_aspects] with ts3[i, a] = sum_qr I[i, q] (sum_p G1[p, q, r] U[u, p]) A[a, r], every sum in
+    f64 and one rounding to f32.  out: an optional [n_q, n_items] f32 device buffer to write."""
+    L_ = require_cuda()
+    for t, name in ((U, "U"), (I, "I"), (A, "A"), (G1, "G1")):
+        _dev(t, torch.float32, name)
+    _dev(user_idx, torch.int64, "user_idx")
+    d1, d2, d3 = (int(x) for x in G1.shape)
+    if (U.dim() != 2 or int(U.shape[1]) != d1 or I.dim() != 2 or int(I.shape[1]) != d2 or A.dim() != 2
+            or int(A.shape[1]) != d3 or A.shape[0] < 2):
+        raise B200Error("U %s, I %s, A %s and G1 %s do not agree in shape"
+                        % (tuple(U.shape), tuple(I.shape), tuple(A.shape), tuple(G1.shape)))
+    n_items = int(I.shape[0]) if n_items is None else int(n_items)
+    if not 0 <= n_items <= int(I.shape[0]):
+        raise B200Error("n_items=%d outside [0, %d]" % (n_items, int(I.shape[0])))
+    n_q = user_idx.numel()
+    if out is None:
+        out = torch.empty((n_q, n_items), dtype=torch.float32, device=U.device)
+    elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()
+              and tuple(out.shape) == (n_q, n_items)):
+        raise B200Error("out must be a contiguous f32 CUDA tensor of shape %s" % ((n_q, n_items),))
+    check(L_.b200_comparer_rank_rows(ptr(U), ptr(I), ptr(A), ptr(G1), ptr(user_idx), n_q, n_items, d1, d2, d3,
+                                     int(A.shape[0]) - 1, int(n_top), float(alpha), ptr(out), current_stream()),
+          "b200_comparer_rank_rows")
+    return out
 
 
 class HpfData(SparseLayout):

@@ -47,7 +47,8 @@ def build_data(train_set, num_users, num_items, rating_scale):
     X holds, for every review (user, item) in `sentiment.user_sentiment` order, the key (u, i, n_aspects) with the
     rating, then the key (u, i, a) of each tuple, in order of first appearance; a tuple key's value is
     1 + (s - 1) / (1 + e^-total), total the f64 sum of its polarities in tuple order.  YU (YI) holds the keys (u, a, o)
-    ((i, a, o)) of the positive tuples in order of first appearance, valued 1 + (s - 1)(2 / (1 + e^-count) - 1)."""
+    ((i, a, o)) of the positive tuples in order of first appearance, valued 1 + (s - 1)(2 / (1 + e^-count) - 1).
+    X64 holds X's f64 values, before the f32 cast (ComparERSub compares them)."""
     sentiment = train_set.sentiment
     n_aspects, n_opinions = int(sentiment.num_aspects), int(sentiment.num_opinions)
     u_idx, i_idx, r_val = train_set.uir_tuple
@@ -113,7 +114,7 @@ def build_data(train_set, num_users, num_items, rating_scale):
     pair_rating = np.asarray(r_val, dtype=np.float64)[last].astype(np.float32)
     assert len(upair) == len(indices)
     return MterData(n_users=int(num_users), n_items=int(num_items), n_aspects=n_aspects, n_opinions=n_opinions,
-                    X=X.astype(np.float32), X_uids=X_uids.astype(np.int32), X_iids=X_iids.astype(np.int32),
+                    X64=X, X=X.astype(np.float32), X_uids=X_uids.astype(np.int32), X_iids=X_iids.astype(np.int32),
                     X_aids=X_aids.astype(np.int32),
                     YU=YU.astype(np.float32), YU_uids=pu[fu].astype(np.int32), YU_aids=pa[fu].astype(np.int32),
                     YU_oids=po[fu].astype(np.int32),
@@ -133,10 +134,11 @@ def check_data(data):
             raise ValueError("MTER cannot sample from an empty %s" % name)
 
 
-def stream_seeds(rng):
+def stream_seeds(rng, n=5):
     """The mt19937 seeds of the five RNGVector streams (uia, uao, iao, pos, neg), in the reference's order: each stream
-    takes self.rng.randint(2**31) and seeds its engine with get_rng(that).randint(2**31) (recom_bpr.pyx:54-59)."""
-    return [int(get_rng(int(rng.randint(2 ** 31))).randint(2 ** 31)) for _ in range(5)]
+    takes self.rng.randint(2**31) and seeds its engine with get_rng(that).randint(2**31) (recom_bpr.pyx:54-59).  n:
+    the number of streams (ComparERSub has six)."""
+    return [int(get_rng(int(rng.randint(2 ** 31))).randint(2 ** 31)) for _ in range(n)]
 
 
 class MTER(DeviceScoringMixin, Recommender):
@@ -229,29 +231,25 @@ class MTER(DeviceScoringMixin, Recommender):
         n_el, n_bpr = int(self.n_element_samples), int(self.n_bpr_samples)
         if n_el < 1 or n_bpr < 1:
             raise ValueError("n_element_samples and n_bpr_samples must be positive")
-        ddata = engine.MterDeviceData(data)
         params = [engine.to_device(np.ascontiguousarray(getattr(self, n)), torch.float32) for n, _ in self._shapes()]
         sgrad = [torch.zeros_like(p) for p in params]
         dims = (self.n_user_factors, self.n_item_factors, self.n_aspect_factors, self.n_opinion_factors)
-        work = torch.zeros(engine.mter_workspace_bytes(ddata, dims, n_el, n_bpr), dtype=torch.uint8, device="cuda")
-        counts = torch.zeros(2, dtype=torch.int64, device="cuda")
-        losses = torch.zeros(2, dtype=torch.float64, device="cuda") if self.verbose else None
-        hyper = dict(lr=self.lr, lambda_reg=self.lambda_reg, lambda_bpr=self.lambda_bpr)
+        counts = torch.zeros(3, dtype=torch.int64, device="cuda")
+        losses = torch.zeros(3, dtype=torch.float64, device="cuda") if self.verbose else None
         seeded = self.seed is not None
-        # seeded: the reference's five streams, drawn on the host; unseeded: Philox on the device, keyed by the first
+        # seeded: the reference's streams, drawn on the host; unseeded: Philox on the device, keyed by the first
         # stream seed, and the rows' gradients summed without a fixed order (the reference's threads define none)
-        draws = MterDraws(seeds, data, n_el, n_bpr, 1 if self.verbose else self.max_iter) if seeded else None
+        fit, draws = self._b200_fit_parts(data, seeds, dims, n_el, n_bpr, 1 if self.verbose else self.max_iter, seeded)
         chunk = 1 if self.verbose else (draws.chunk if seeded else self.max_iter)
         done = 0
         while done < self.max_iter:
             n = min(chunk, self.max_iter - done)
-            engine.mter_fit(ddata, params, sgrad, draws.next(n) if seeded else None, n, n_el, n_bpr, counts=counts,
-                            losses=losses, workspace=work, unordered=not seeded,
-                            philox_seed=None if seeded else seeds[0], iter0=done, **hyper)
+            fit(params, sgrad, draws.next(n) if seeded else None, n, counts=counts, losses=losses,
+                unordered=not seeded, philox_seed=None if seeded else seeds[0], iter0=done)
             done += n
             if self.verbose:
-                correct, skipped = counts.tolist()
-                loss, bpr_loss = losses.tolist()
+                correct, skipped = counts.tolist()[:2]
+                loss, bpr_loss = losses.tolist()[:2]
                 print("iter %d: loss %.2f, bpr_loss %.2f, correct %.2f%%, skipped %.2f%%"
                       % (done, loss / 3 / n_el, bpr_loss / n_bpr,
                          100.0 * correct / max(n_bpr - skipped, 1), 100.0 * skipped / n_bpr))
@@ -261,6 +259,17 @@ class MTER(DeviceScoringMixin, Recommender):
             print("Optimization finished!")
         for (name, _), d in zip(self._shapes(), params):
             setattr(self, name, _copy_back(getattr(self, name), d))
+
+    def _b200_fit_parts(self, data, seeds, dims, n_el, n_bpr, max_chunk, seeded):
+        """(fit, draws) of _fit_b200: fit(params, sgrad, draws, n_iter, **kw) runs n_iter iterations of the device fit
+        over this fit's device data and workspace; draws is the MterDraws of the seeded streams, or None."""
+        ddata = engine.MterDeviceData(data)
+        work = torch.zeros(engine.mter_workspace_bytes(ddata, dims, n_el, n_bpr), dtype=torch.uint8, device="cuda")
+        hyper = dict(lr=self.lr, lambda_reg=self.lambda_reg, lambda_bpr=self.lambda_bpr)
+
+        def fit(params, sgrad, draws, n, **kw):
+            engine.mter_fit(ddata, params, sgrad, draws, n, n_el, n_bpr, workspace=work, **hyper, **kw)
+        return fit, (MterDraws(seeds, data, n_el, n_bpr, max_chunk) if seeded else None)
 
     # ---- device scoring: U := Q (the rank queries of every user), V := I --------------------------------------------
     def _b200_device(self):

@@ -674,6 +674,45 @@ B200_API int b200_mter_queries(const float* U, int64_t n_users, const float* G1,
                                int d3, float* Q, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * ComparERSub (cornac/models/comparer/recom_comparer_sub.pyx:487-806): MTER plus a third sample phase over the
+ * comparative pairs (user, earlier item, later item, aspect) of the user's purchase history.
+ *
+ * b200_comparer_sub_fit: b200_mter_fit's fit and arguments (b200_mter_fit is the case n_pair = 0), plus
+ *   p_user, p_earlier, p_later, p_aspect   int32 [n_plist]: the pair list, in the reference's order
+ *   n_pair            pair samples per iteration (>= 0; n_plist > 0 when n_pair > 0)
+ *   draws             int32 [n_iter][3 n_el + 2 n_bpr + n_pair]: b200_mter_fit's draws of an iteration, then the
+ *                     n_pair draws of the pair stream
+ *   lambda_d          f32, the weight of the pair terms
+ *   work              device, b200_comparer_sub_workspace_bytes(...) bytes, zero before the first call
+ *   counts            device u64[3]: += correct, skipped, aspect_correct (pairs whose later item scores higher)
+ *   losses            device f64[3] or NULL: += loss, bpr_loss, aspect_bpr_loss
+ * A pair sample's terms follow the BPR samples' in every accumulator chain; within a sample with earlier == later the
+ * I row takes -v then +v for every term, as the reference's statements do.
+ *
+ * b200_comparer_rank_rows: out [n_q, n_items] f32, the rank rows of users[0..n_q) over items [0, n_items):
+ *   ts3[i, a] = sum_q I[i, q] sum_r (sum_p G1[p, q, r] U[u, p]) A[a, r] for a <= n_aspects, and
+ *   out[i] = f32(alpha * mean(the n_top largest ts3[i, a < n_aspects]) + (1 - alpha) * ts3[i, n_aspects]),
+ *   every sum in f64 in index order and one rounding at the end (0 < n_top <= n_aspects < 1024).                       */
+B200_API int64_t b200_comparer_sub_workspace_bytes(int64_t n_users, int64_t n_items, int64_t n_aspects,
+                                                   int64_t n_opinions, int d1, int d2, int d3, int d4, int n_el,
+                                                   int n_bpr, int n_pair);
+B200_API int b200_comparer_sub_fit(int64_t n_users, int64_t n_items, int64_t n_aspects, int64_t n_opinions, int d1,
+                                   int d2, int d3, int d4, const float* X, const int32_t* X_u, const int32_t* X_i,
+                                   const int32_t* X_a, int64_t n_x, const float* YU, const int32_t* YU_u,
+                                   const int32_t* YU_a, const int32_t* YU_o, int64_t n_yu, const float* YI,
+                                   const int32_t* YI_i, const int32_t* YI_a, const int32_t* YI_o, int64_t n_yi,
+                                   const int32_t* indptr, const int32_t* indices, const int32_t* rrow,
+                                   const float* rval, int64_t nnz, const int32_t* p_user, const int32_t* p_earlier,
+                                   const int32_t* p_later, const int32_t* p_aspect, int64_t n_plist, int n_el,
+                                   int n_bpr, int n_pair, int n_iter, const int32_t* draws, float* const* params,
+                                   float* const* sgrad, void* work, float lr, float lambda_reg, float lambda_bpr,
+                                   float lambda_d, int flags, uint64_t seed, uint64_t iter0, unsigned long long* counts,
+                                   double* losses, unsigned long long* phase_ns, void* stream);
+B200_API int b200_comparer_rank_rows(const float* U, const float* I, const float* A, const float* G1,
+                                     const int64_t* users, int64_t n_q, int64_t n_items, int d1, int d2, int d3,
+                                     int64_t n_aspects, int n_top, double alpha, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Multi-GPU item-factor exchange (no reference counterpart: the reference is a single
  * process).  Each rank trains its user shard against a replica of V / B; at the epoch
  * boundary   b200_delta_make:  delta[i] = x[i] - snapshot[i]
