@@ -44,10 +44,53 @@ def warmup():
     return L
 
 
-def _dev(t, dtype, name):
-    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous()):
-        raise B200Error("%s must be a contiguous CUDA tensor of dtype %s" % (name, dtype))
-    return t
+class _AtLeast(int):
+    """A minimum size in a shape _dev checks: the kernel reads only a prefix of that extent."""
+
+
+def _fits(n, want):
+    return want is None or (n >= want if type(want) is _AtLeast else n == want)
+
+
+def _size_str(want):
+    return "*" if want is None else (">=%d" if type(want) is _AtLeast else "%d") % want
+
+
+def _dev(t, dtype, name, shape=None):
+    """t, checked to be a contiguous CUDA tensor of `dtype` and, when `shape` is given, of that shape: a tuple with per
+    dimension an exact size, an _AtLeast or None (any size); or one size (exact or _AtLeast), the element count of a
+    flat buffer.  The C entry points take raw pointers: these are the only checks of the extents they index."""
+    if isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous():
+        if shape is None:
+            return t
+        if type(shape) is not tuple:
+            if _fits(t.numel(), shape):
+                return t
+        elif len(t.shape) == len(shape) and all(map(_fits, t.shape, shape)):
+            return t
+    if shape is None:
+        want = ""
+    elif isinstance(shape, tuple):
+        want = " and shape (%s)" % ", ".join(map(_size_str, shape))
+    else:
+        want = " and shape [%s elements]" % _size_str(shape)
+    got = ("a %s tensor of dtype %s and shape %s" % (t.device, t.dtype, tuple(t.shape)) if isinstance(t, torch.Tensor)
+           else type(t).__name__)
+    raise B200Error("%s must be a contiguous CUDA tensor of dtype %s%s, got %s" % (name, dtype, want, got))
+
+
+def _buf(t, dtype, name, shape, zero=False):
+    """An optional caller buffer: t checked by _dev when given, else a new CUDA tensor of `shape` (zeros when `zero`;
+    a flat buffer gets at least one element, as no device buffer here is zero-size)."""
+    if t is None:
+        return (torch.zeros if zero else torch.empty)(shape if isinstance(shape, tuple) else max(int(shape), 1),
+                                                      dtype=dtype, device="cuda")
+    return _dev(t, dtype, name, shape)
+
+
+def _f32(x):
+    """x rounded to f32, as the reference's C `float` / `floating` parameters hold it."""
+    return float(np.float32(x))
 
 
 def to_device(a, dtype=None, pinned=True):
@@ -76,9 +119,7 @@ class BprData:
         self.indices = _dev(indices, torch.int32, "indices")
         self.n_users = self.indptr.numel() - 1
         self.nnz = self.indices.numel()
-        self._coo_row = None if coo_row is None else _dev(coo_row, torch.int32, "coo_row")
-        if self._coo_row is not None and self._coo_row.numel() != self.nnz:
-            raise B200Error("coo_row length %d != nnz %d" % (self._coo_row.numel(), self.nnz))
+        self._coo_row = None if coo_row is None else _dev(coo_row, torch.int32, "coo_row", self.nnz)
         self.pairs = self.table = None
 
     @property
@@ -115,9 +156,9 @@ def bpr_epoch(data, n_neg, U, V, B, lr, reg, use_bias, seed, epoch, stats, n_sam
     (correct, skipped).  deterministic=True: rounds of samples that read the factors as the previous round left them,
     their updates summed exactly -- the result repeats bit for bit from run to run."""
     L = require_cuda()
-    k = U.shape[1]
-    _dev(U, torch.float32, "U"), _dev(V, torch.float32, "V"), _dev(B, torch.float32, "B")
-    _dev(stats, torch.int64, "stats")
+    k = _dev(U, torch.float32, "U", (_AtLeast(data.n_users), None)).shape[1]
+    _dev(V, torch.float32, "V", (_AtLeast(n_neg), k)), _dev(B, torch.float32, "B", _AtLeast(n_neg))
+    _dev(stats, torch.int64, "stats", _AtLeast(2))
     flags = ((_lib.SGD_ATOMIC if atomic else 0) | (_lib.SGD_EXACT_EXP if exact_exp else 0)
              | (_lib.SGD_UNBOUNDED if unbounded else 0) | (_lib.BPR_NEG_WEIGHTED if neg_weighted else 0)
              | (_lib.BPR_LOSS_HINGE if hinge else 0) | (_lib.BPR_BLOCKED if blocked else 0)
@@ -153,12 +194,14 @@ def bpr_draw_host(seed, epoch, n, nnz, n_neg, sample_base=0, plan=(1, 1)):
 def bpr_epoch_replay(data, i_index, j_id, U, V, B, lr, reg, use_bias, stats, hinge=False):
     """Serial-equivalent application of an explicit sample stream (parity mode)."""
     L = require_cuda()
-    _dev(i_index, torch.int64, "i_index"), _dev(j_id, torch.int32, "j_id")
-    _dev(U, torch.float32, "U"), _dev(V, torch.float32, "V"), _dev(B, torch.float32, "B")
-    check(L.b200_bpr_epoch_replay2(ptr(i_index), ptr(j_id), i_index.numel(), ptr(data.indptr), ptr(data.indices),
-                                   ptr(data.coo_row), int(U.shape[0]), int(V.shape[0]), ptr(U), ptr(V), ptr(B), int(U.shape[1]),
-                                   float(lr), float(reg), int(bool(use_bias)), _lib.BPR_LOSS_HINGE if hinge else 0,
-                                   ptr(_dev(stats, torch.int64, "stats")), current_stream()),
+    n = _dev(i_index, torch.int64, "i_index").numel()
+    _dev(j_id, torch.int32, "j_id", _AtLeast(n))
+    k = _dev(U, torch.float32, "U", (_AtLeast(data.n_users), None)).shape[1]
+    n_items = _dev(V, torch.float32, "V", (None, k)).shape[0]
+    _dev(B, torch.float32, "B", _AtLeast(n_items)), _dev(stats, torch.int64, "stats", _AtLeast(2))
+    check(L.b200_bpr_epoch_replay2(ptr(i_index), ptr(j_id), n, ptr(data.indptr), ptr(data.indices), ptr(data.coo_row),
+                                   int(U.shape[0]), int(n_items), ptr(U), ptr(V), ptr(B), int(k), float(lr), float(reg),
+                                   int(bool(use_bias)), _lib.BPR_LOSS_HINGE if hinge else 0, ptr(stats), current_stream()),
           "b200_bpr_epoch_replay")
 
 
@@ -190,7 +233,7 @@ def bpr_train_host(indptr, indices, n_neg, U, V, B, lr, reg, use_bias, max_iter,
     for t in (dU, dV, dB):
         t.record_stream(main)
     stats = torch.zeros(2, dtype=torch.int64, device="cuda")
-    lr, reg = float(np.float32(lr)), float(np.float32(reg))
+    lr, reg = _f32(lr), _f32(reg)
     history = []
     sync = None
     if replica_sync:
@@ -276,19 +319,18 @@ def tri_train_host(kind, indptr, indices, aux, n_items, U, V, B, hyper, max_iter
     n_users, k = int(dU.shape[0]), int(dU.shape[1])
     max_iter = int(max_iter)
     stats_all = torch.zeros((max(max_iter, 1), 2), dtype=torch.int64, device="cuda")
-    f32 = lambda x: float(np.float32(x))          # noqa: E731
     st = current_stream
 
     def hogwild(epoch):
         if kind == "vebpr":
             check(L.b200_vebpr_epoch(ptr(data.indptr), ptr(data.indices), ptr(coo), n_users, int(n_items), nnz,
-                                     ptr(aux_dev[0]), ptr(aux_dev[1]), ptr(dU), ptr(dV), k, f32(hyper["lr"]), f32(hyper["reg"]),
-                                     f32(hyper["alpha"]), int(key) & ((1 << 64) - 1), epoch, nnz, ptr(stats_all[epoch]), st()),
+                                     ptr(aux_dev[0]), ptr(aux_dev[1]), ptr(dU), ptr(dV), k, _f32(hyper["lr"]), _f32(hyper["reg"]),
+                                     _f32(hyper["alpha"]), int(key) & ((1 << 64) - 1), epoch, nnz, ptr(stats_all[epoch]), st()),
                   "b200_vebpr_epoch")
         else:
             check(L.b200_sbpr_epoch(ptr(data.indptr), ptr(data.indices), ptr(coo), n_users, int(n_items), nnz,
                                     ptr(aux_dev[0]), ptr(aux_dev[1]), ptr(aux_dev[2]), len(aux[1]), ptr(dU), ptr(dV), ptr(dB), k,
-                                    f32(hyper["lr"]), f32(hyper["lambda_u"]), f32(hyper["lambda_v"]), f32(hyper["lambda_b"]),
+                                    _f32(hyper["lr"]), _f32(hyper["lambda_u"]), _f32(hyper["lambda_v"]), _f32(hyper["lambda_b"]),
                                     int(bool(hyper["use_bias"])), int(key) & ((1 << 64) - 1), epoch, nnz, ptr(stats_all[epoch]), st()),
                   "b200_sbpr_epoch")
 
@@ -326,12 +368,12 @@ def tri_train_host(kind, indptr, indices, aux, n_items, U, V, B, hyper, max_iter
             fence[b].record()
             if kind == "vebpr":
                 check(L.b200_vebpr_epoch_replay(ptr(d_i[b]), ptr(d_t[b]), ptr(d_j[b]), nnz, ptr(data.indptr), ptr(data.indices), ptr(coo),
-                                                ptr(aux_dev[0]), ptr(aux_dev[1]), ptr(dU), ptr(dV), k, f32(hyper["lr"]), f32(hyper["reg"]),
-                                                f32(hyper["alpha"]), ptr(stats_all[epoch]), st()), "b200_vebpr_epoch_replay")
+                                                ptr(aux_dev[0]), ptr(aux_dev[1]), ptr(dU), ptr(dV), k, _f32(hyper["lr"]), _f32(hyper["reg"]),
+                                                _f32(hyper["alpha"]), ptr(stats_all[epoch]), st()), "b200_vebpr_epoch_replay")
             else:
                 check(L.b200_sbpr_epoch_replay(ptr(d_i[b]), ptr(d_j[b]), ptr(d_t[b]), nnz, ptr(data.indptr), ptr(data.indices), ptr(coo),
                                                ptr(aux_dev[0]), ptr(aux_dev[1]), ptr(aux_dev[2]), len(aux[1]), ptr(dU), ptr(dV), ptr(dB), k,
-                                               f32(hyper["lr"]), f32(hyper["lambda_u"]), f32(hyper["lambda_v"]), f32(hyper["lambda_b"]),
+                                               _f32(hyper["lr"]), _f32(hyper["lambda_u"]), _f32(hyper["lambda_v"]), _f32(hyper["lambda_b"]),
                                                int(bool(hyper["use_bias"])), ptr(stats_all[epoch]), st()), "b200_sbpr_epoch_replay")
             if on_epoch:
                 on_epoch(epoch, *stats_all[epoch].cpu().tolist())
@@ -390,15 +432,17 @@ def mf_epoch(rid, cid, val, U, V, Bu, Bi, lr, reg, mu, use_bias, loss, ordered=F
     L = require_cuda()
     if rid.dtype not in (torch.int32, torch.int64) or cid.dtype != rid.dtype:
         raise B200Error("rid/cid must both be int32 or int64")
-    _dev(rid, rid.dtype, "rid"), _dev(cid, rid.dtype, "cid"), _dev(val, torch.float32, "val")
-    for n_, t_ in (("U", U), ("V", V), ("Bu", Bu), ("Bi", Bi), ("loss", loss)):
-        if t_ is not None or n_ not in ("U", "V"):
-            _dev(t_, torch.float32, n_)
     if (U is None) != (V is None):
         raise B200Error("U and V must both be given or both be None")
-    k = 0 if U is None else int(U.shape[1])
-    check(L.b200_mf_epoch(ptr(rid), ptr(cid), ptr(val), val.numel(), int(rid.dtype == torch.int32),
-                          int(Bu.shape[0]), int(Bi.shape[0]), ptr(U), ptr(V), ptr(Bu), ptr(Bi), k, float(lr), float(reg), float(mu),
+    n = _dev(val, torch.float32, "val").numel()
+    _dev(rid, rid.dtype, "rid", _AtLeast(n)), _dev(cid, rid.dtype, "cid", _AtLeast(n))
+    n_users, n_items = _dev(Bu, torch.float32, "Bu").numel(), _dev(Bi, torch.float32, "Bi").numel()
+    _dev(loss, torch.float32, "loss", _AtLeast(1))
+    k = 0 if U is None else _dev(U, torch.float32, "U", (_AtLeast(n_users), None)).shape[1]
+    if V is not None:
+        _dev(V, torch.float32, "V", (_AtLeast(n_items), k))
+    check(L.b200_mf_epoch(ptr(rid), ptr(cid), ptr(val), n, int(rid.dtype == torch.int32),
+                          n_users, n_items, ptr(U), ptr(V), ptr(Bu), ptr(Bi), int(k), float(lr), float(reg), float(mu),
                           int(bool(use_bias)), int(bool(ordered)),
                           (_lib.SGD_ATOMIC if atomic else 0) | (_lib.SGD_UNBOUNDED if unbounded else 0), ptr(loss),
                           current_stream()), "b200_mf_epoch")
@@ -418,14 +462,12 @@ class WmfTrainer:
         if csc.nnz >= 2 ** 31:
             raise B200Error("nnz >= 2^31 is not supported (int32 CSC offsets)")
         self.n_users, self.n_items = (int(x) for x in csc.shape)
-        if U.shape[0] != self.n_users or V.shape[0] != self.n_items or U.shape[1] != V.shape[1]:
-            raise B200Error("U / V shapes %s / %s do not match the %d x %d rating matrix" % (U.shape, V.shape, self.n_users, self.n_items))
-        self.k = int(U.shape[1])
+        self.U = _dev(to_device(np.ascontiguousarray(U, dtype=np.float32)), torch.float32, "U", (self.n_users, None))
+        self.k = int(self.U.shape[1])
+        self.V = _dev(to_device(np.ascontiguousarray(V, dtype=np.float32)), torch.float32, "V", (self.n_items, self.k))
         self.indptr = to_device(csc.indptr, torch.int32)
         self.rows = to_device(csc.indices if csc.nnz else np.zeros(1, np.int32), torch.int32)
         self.vals = to_device(np.asarray(csc.data if csc.nnz else np.zeros(1), dtype=np.float32), torch.float32)
-        self.U = to_device(np.ascontiguousarray(U, dtype=np.float32), torch.float32)
-        self.V = to_device(np.ascontiguousarray(V, dtype=np.float32), torch.float32)
         self.mU, self.vU = torch.zeros_like(self.U), torch.zeros_like(self.U)
         self.mV, self.vV = torch.zeros_like(self.V), torch.zeros_like(self.V)
         self.slot_of = torch.full((self.n_items,), -1, dtype=torch.int32, device="cuda")
@@ -453,7 +495,7 @@ class WmfTrainer:
         lr_t = self.lr * np.sqrt(f32(1) - self.b2_pow) / (f32(1) - self.b1_pow)          # AdamOptimizer._prepare / _apply_*
         check(L.b200_wmf_step(ptr(self.indptr), ptr(self.rows), ptr(self.vals), ptr(d_ids), b, self.n_users, self.n_items,
                               self.k, ptr(self.U), ptr(self.V), ptr(self.mU), ptr(self.vU), ptr(self.mV), ptr(self.vV),
-                              float(self.a), float(self.b), float(self.lambda_u), float(self.lambda_v), float(f32(lr_t)),
+                              float(self.a), float(self.b), float(self.lambda_u), float(self.lambda_v), _f32(lr_t),
                               self.BETA1, self.BETA2, self.EPS, ptr(self.slot_of), ptr(self.gV), ptr(self.loss),
                               current_stream()), "b200_wmf_step")
         self.b1_pow = f32(self.b1_pow * f32(self.BETA1))              # _finish: the beta powers advance once per step
@@ -565,12 +607,9 @@ def ease_gram(inp, lamb, out, workspace=None):
     raw mode of the KNN similarity kernel over the rows of X^T).  inp: EaseGramInput of X."""
     L = require_cuda()
     n = inp.n
-    _dev(out, torch.float64, "out")
-    if tuple(out.shape) != (n, n):
-        raise B200Error("out must have shape (%d, %d)" % (n, n))
+    _dev(out, torch.float64, "out", (n, n))
     ws_bytes = int(L.b200_ease_gram_workspace_bytes(n))
-    if workspace is None and ws_bytes:
-        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
+    workspace = _buf(workspace, torch.uint8, "workspace", _AtLeast(ws_bytes))
     (r_p, r_i, r_d), (c_p, c_i, c_d) = inp.rows, inp.cols
     check(L.b200_ease_gram(n, ptr(r_p), ptr(r_i), ptr(r_d), max(inp.n_users, 1), ptr(c_p), ptr(c_i), ptr(c_d),
                            ptr(inp.order), float(lamb), ptr(workspace) if ws_bytes else None, ptr(out), current_stream()),
@@ -584,14 +623,10 @@ def spd_inverse(A, phases=_lib.SPD_ALL, workspace=None, info=None):
     workspace and info).  Raises numpy.linalg.LinAlgError naming the first failing column when A is not positive definite
     (checked after the factorisation; the call then synchronises with the device)."""
     L = require_cuda()
-    _dev(A, torch.float64, "A")
-    n = int(A.shape[0])
-    if A.dim() != 2 or int(A.shape[1]) != n:
-        raise B200Error("A must be square, got %s" % (tuple(A.shape),))
-    if workspace is None:
-        workspace = torch.empty(int(L.b200_spd_inverse_workspace_bytes(n)), dtype=torch.uint8, device="cuda")
-    if info is None:
-        info = torch.zeros(1, dtype=torch.int32, device="cuda")
+    n = _dev(A, torch.float64, "A", (None, None)).shape[0]
+    _dev(A, torch.float64, "A", (n, n))
+    workspace = _buf(workspace, torch.uint8, "workspace", _AtLeast(L.b200_spd_inverse_workspace_bytes(n)))
+    info = _buf(info, torch.int32, "info", _AtLeast(1), zero=True)
     check(L.b200_spd_inverse(n, ptr(A), ptr(workspace), ptr(info), int(phases), current_stream()), "b200_spd_inverse")
     if phases & _lib.SPD_POTRF:
         bad = int(info.item())
@@ -604,10 +639,9 @@ def spd_inverse(A, phases=_lib.SPD_ALL, workspace=None, info=None):
 def ease_weights(P, posB, diag=None):
     """B = P / -diag(P), B[j, j] = 0, negatives to 0 under posB, in place on the f64 device matrix P (b200_ease_weights)."""
     L = require_cuda()
-    _dev(P, torch.float64, "P")
-    n = int(P.shape[0])
-    if diag is None:
-        diag = torch.empty(n, dtype=torch.float64, device="cuda")
+    n = _dev(P, torch.float64, "P", (None, None)).shape[0]
+    _dev(P, torch.float64, "P", (n, n))
+    diag = _buf(diag, torch.float64, "diag", _AtLeast(n))
     check(L.b200_ease_weights(n, ptr(P), ptr(diag), int(bool(posB)), current_stream()), "b200_ease_weights")
     return P
 
@@ -646,10 +680,8 @@ def ease_score(B, users, ratings, out=None):
     """out[q, :] = X[users[q], :] . B in scipy's order (b200_ease_score): f64 [n_q, n_items] device score rows.
     ratings: EaseRatings of X; B: f64 device [n_items, n_items]; users: indices of rows of X (host or int64 device)."""
     L = require_cuda()
-    _dev(B, torch.float64, "B")
-    n = int(B.shape[0])
-    if B.dim() != 2 or int(B.shape[1]) != n or n != ratings.n_cols:
-        raise B200Error("B must be square with one row per item of the ratings (%d), got %s" % (ratings.n_cols, tuple(B.shape)))
+    n = ratings.n_cols
+    _dev(B, torch.float64, "B", (n, n))
     if isinstance(users, torch.Tensor):
         _dev(users, torch.int64, "users")
         lo, hi = (int(users.min()), int(users.max())) if users.numel() else (0, 0)
@@ -660,10 +692,9 @@ def ease_score(B, users, ratings, out=None):
     if lo < 0 or hi >= ratings.n_rows:
         raise B200Error("user index out of range [0, %d): %d" % (ratings.n_rows, lo if lo < 0 else hi))
     n_q = int(users.numel())
-    if out is None:
-        out = torch.empty((n_q, n), dtype=torch.float64, device="cuda")
+    out = _buf(out, torch.float64, "out", (n_q, n))
     check(L.b200_ease_score(ptr(users), n_q, n, ptr(ratings.indptr), ptr(ratings.indices), ptr(ratings.data), ptr(B),
-                            ptr(_dev(out, torch.float64, "out")), current_stream()), "b200_ease_score")
+                            ptr(out), current_stream()), "b200_ease_score")
     return out
 
 
@@ -699,14 +730,15 @@ def knn_score(user_mode, S, users, ratings, k):
     f64 [n_q, n_items] device scores.  user_mode: UserKNN (S is [n_users, n_users], ratings the item-user matrix);
     otherwise ItemKNN (S is [n_items, n_items], ratings the user-item matrix)."""
     L = require_cuda()
-    _dev(S, torch.float64, "S")
+    n = ratings.n_cols                            # the similarity's rows and columns are the ratings' columns
+    _dev(S, torch.float64, "S", (n, n))
     if k < 1:
         raise B200Error("k must be >= 1, got %d" % k)
     users = users if isinstance(users, torch.Tensor) else to_device(np.asarray(users, dtype=np.int64), torch.int64)
     _dev(users, torch.int64, "users")
     n_q = int(users.numel())
-    n_users = int(S.shape[0]) if user_mode else ratings.n_rows
-    n_items = ratings.n_rows if user_mode else int(S.shape[0])
+    n_users = n if user_mode else ratings.n_rows
+    n_items = ratings.n_rows if user_mode else n
     out = torch.empty((n_q, n_items), dtype=torch.float64, device="cuda")
     ws_bytes = int(L.b200_knn_score_workspace_bytes(n_q, n_users if user_mode else 0, int(k)))
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda") if ws_bytes else None
@@ -723,28 +755,41 @@ def knn_score(user_mode, S, users, ratings, k):
 def score_batch(U, V, user_idx=None, item_base=None, user_off=None, n_items=None, out=None):
     """out[q, i] = (item_base[i] + user_off[q]) + dot(U[user_idx[q]], V[i]) for i < n_items."""
     L = require_cuda()
-    _dev(U, torch.float32, "U"), _dev(V, torch.float32, "V")
-    n_items = V.shape[0] if n_items is None else int(n_items)
-    n_q = U.shape[0] if user_idx is None else user_idx.numel()
-    if user_idx is not None:
-        _dev(user_idx, torch.int64, "user_idx")
-    if out is None:
-        out = torch.empty((n_q, n_items), dtype=torch.float32, device=U.device)
-    check(L.b200_score_batch(ptr(U), ptr(user_idx), n_q, ptr(V), n_items, int(V.shape[1]), ptr(item_base),
-                             ptr(user_off), ptr(_dev(out, torch.float32, "out")), current_stream()),
-          "b200_score_batch")
+    n_items, k, n_q = _score_args(U, V, user_idx, n_items, torch.float32, item_base, user_off)
+    out = _buf(out, torch.float32, "out", (n_q, n_items))
+    check(L.b200_score_batch(ptr(U), ptr(user_idx), n_q, ptr(V), n_items, k, ptr(item_base), ptr(user_off), ptr(out),
+                             current_stream()), "b200_score_batch")
     return out
+
+
+def _score_args(U, V, user_idx, n_items, dtype, item_base=None, user_off=None):
+    """(n_items, k, n_q) of a score or rank call, checked: V [>= n_items (default all rows), k], U [*, k] (its rows the
+    queries when user_idx is None), user_idx int64 [n_q], item_base [>= n_items] and user_off [>= n_q] when given."""
+    k = _dev(V, dtype, "V", (None if n_items is None else _AtLeast(n_items), None)).shape[1]
+    n_items = int(V.shape[0] if n_items is None else n_items)
+    _dev(U, dtype, "U", (None, k))
+    n_q = U.shape[0] if user_idx is None else _dev(user_idx, torch.int64, "user_idx").numel()
+    if item_base is not None:
+        _dev(item_base, dtype, "item_base", _AtLeast(n_items))
+    if user_off is not None:
+        _dev(user_off, dtype, "user_off", _AtLeast(n_q))
+    return n_items, int(k), int(n_q)
+
+
+def _exclusions(excl_indptr, excl_indices, n_q):
+    """Checks the optional per-row exclusion CSR: excl_indptr int64 [>= n_q + 1], excl_indices int32."""
+    if excl_indptr is not None:
+        _dev(excl_indptr, torch.int64, "excl_indptr", _AtLeast(n_q + 1))
+        _dev(excl_indices, torch.int32, "excl_indices")
 
 
 def topk_rows(scores, topk, excl_indptr=None, excl_indices=None):
     """Exact top-k (score desc, id asc) of each row of `scores`, with per-row exclusions."""
     L = require_cuda()
-    _dev(scores, torch.float32, "scores")
-    n_q, n_items = scores.shape
+    n_q, n_items = _dev(scores, torch.float32, "scores", (None, None)).shape
     ids = torch.empty((n_q, topk), dtype=torch.int32, device=scores.device)
     sc = torch.empty((n_q, topk), dtype=torch.float32, device=scores.device)
-    if excl_indptr is not None:
-        _dev(excl_indptr, torch.int64, "excl_indptr"), _dev(excl_indices, torch.int32, "excl_indices")
+    _exclusions(excl_indptr, excl_indices, n_q)
     check(L.b200_topk_rows(ptr(scores), n_q, n_items, ptr(excl_indptr), ptr(excl_indices), int(topk), ptr(ids),
                            ptr(sc), current_stream()), "b200_topk_rows")
     return ids, sc
@@ -753,27 +798,20 @@ def topk_rows(scores, topk, excl_indptr=None, excl_indices=None):
 def score_batch_f64(U, V, user_idx=None, n_items=None, out=None):
     """out[q, i] = sum_f U[user_idx[q], f] * V[i, f] in f64 (f ascending, no FMA) for i < n_items."""
     L = require_cuda()
-    _dev(U, torch.float64, "U"), _dev(V, torch.float64, "V")
-    n_items = V.shape[0] if n_items is None else int(n_items)
-    n_q = U.shape[0] if user_idx is None else user_idx.numel()
-    if user_idx is not None:
-        _dev(user_idx, torch.int64, "user_idx")
-    if out is None:
-        out = torch.empty((n_q, n_items), dtype=torch.float64, device=U.device)
-    check(L.b200_score_batch_f64(ptr(U), ptr(user_idx), n_q, ptr(V), n_items, int(V.shape[1]),
-                                 ptr(_dev(out, torch.float64, "out")), current_stream()), "b200_score_batch_f64")
+    n_items, k, n_q = _score_args(U, V, user_idx, n_items, torch.float64)
+    out = _buf(out, torch.float64, "out", (n_q, n_items))
+    check(L.b200_score_batch_f64(ptr(U), ptr(user_idx), n_q, ptr(V), n_items, k, ptr(out), current_stream()),
+          "b200_score_batch_f64")
     return out
 
 
 def topk_rows_f64(scores, topk, excl_indptr=None, excl_indices=None):
     """topk_rows over f64 score rows: exact top-k (score desc, id asc) with per-row exclusions."""
     L = require_cuda()
-    _dev(scores, torch.float64, "scores")
-    n_q, n_items = scores.shape
+    n_q, n_items = _dev(scores, torch.float64, "scores", (None, None)).shape
     ids = torch.empty((n_q, topk), dtype=torch.int32, device=scores.device)
     sc = torch.empty((n_q, topk), dtype=torch.float64, device=scores.device)
-    if excl_indptr is not None:
-        _dev(excl_indptr, torch.int64, "excl_indptr"), _dev(excl_indices, torch.int32, "excl_indices")
+    _exclusions(excl_indptr, excl_indices, n_q)
     check(L.b200_topk_rows_f64(ptr(scores), n_q, n_items, ptr(excl_indptr), ptr(excl_indices), int(topk), ptr(ids),
                                ptr(sc), current_stream()), "b200_topk_rows_f64")
     return ids, sc
@@ -802,7 +840,7 @@ class PmfData:
 
     def __init__(self, uid, iid, rat, n_users, n_items):
         require_cuda()
-        self.nnz = len(uid)
+        self.nnz, self.n_users, self.n_items = len(uid), int(n_users), int(n_items)
         self.order_host, level_ptr = pmf_schedule(uid, iid, n_users, n_items)
         self.n_levels = len(level_ptr) - 1
         o = self.order_host
@@ -821,17 +859,14 @@ def pmf_fit(data, variant, U, V, cache_u, cache_v, n_epochs, lambda_reg, learnin
     variants = {"linear": _lib.PMF_LINEAR, "non_linear": _lib.PMF_NON_LINEAR}
     if variant not in variants:
         raise B200Error('variant must be one of {"linear","non_linear"}, got %r' % (variant,))
-    k = int(U.shape[1])
-    for t, name in ((U, "U"), (V, "V"), (cache_u, "cache_u"), (cache_v, "cache_v")):
-        _dev(t, torch.float64, name)
-        if t.dim() != 2 or int(t.shape[1]) != k:
-            raise B200Error("%s must be 2-D with %d columns" % (name, k))
+    users, items = _AtLeast(data.n_users), _AtLeast(data.n_items)
+    k = _dev(U, torch.float64, "U", (users, None)).shape[1]
+    _dev(cache_u, torch.float64, "cache_u", (users, k))
+    _dev(V, torch.float64, "V", (items, k)), _dev(cache_v, torch.float64, "cache_v", (items, k))
     if loss is not None:
-        _dev(loss, torch.float64, "loss")
-        if loss.numel() != int(n_epochs) * data.nnz:
-            raise B200Error("loss must hold n_epochs * nnz = %d values" % (int(n_epochs) * data.nnz))
+        _dev(loss, torch.float64, "loss", (int(n_epochs), data.nnz))
     check(L.b200_pmf_fit(variants[variant], ptr(data.uid), ptr(data.iid), ptr(data.rat), ptr(data.level_ptr),
-                         data.n_levels, data.nnz, k, ptr(U), ptr(V), ptr(cache_u), ptr(cache_v), int(n_epochs),
+                         data.n_levels, data.nnz, int(k), ptr(U), ptr(V), ptr(cache_u), ptr(cache_v), int(n_epochs),
                          float(lambda_reg), float(learning_rate), float(gamma), ptr(loss),
                          ptr(data.order) if loss is not None else None, current_stream()), "b200_pmf_fit")
 
@@ -878,6 +913,7 @@ class CofactorData:
         require_cuda()
         self.variant = variant
         self.n_edges, self.n_ratings = len(net_a), len(uid)
+        self.n_users, self.n_items = int(n_users), int(n_items)
         if len(net_val) != self.n_edges or len(rat) != self.n_ratings:
             raise B200Error("net_val has %d values for %d edges, rat %d for %d ratings"
                             % (len(net_val), self.n_edges, len(rat), self.n_ratings))
@@ -900,18 +936,16 @@ def cofactor_fit(data, U, V, Z, cache_u, cache_v, cache_z, n_epochs, lambda_c, l
     the reference's C floats.  loss: optional f64 device tensor [n_epochs, n_edges + n_ratings] that receives each
     update's loss term at its stored index."""
     L = require_cuda()
-    k = int(U.shape[1])
-    for t, name in ((U, "U"), (V, "V"), (Z, "Z"), (cache_u, "cache_u"), (cache_v, "cache_v"), (cache_z, "cache_z")):
-        _dev(t, torch.float64, name)
-        if t.dim() != 2 or int(t.shape[1]) != k:
-            raise B200Error("%s must be 2-D with %d columns" % (name, k))
-    n_total = data.n_edges + data.n_ratings
+    users, items = _AtLeast(data.n_users), _AtLeast(data.n_items)
+    z_rows = users if data.variant == "sorec" else items             # SoRec's Z rows are users, MCF's items
+    k = _dev(U, torch.float64, "U", (users, None)).shape[1]
+    _dev(cache_u, torch.float64, "cache_u", (users, k))
+    _dev(V, torch.float64, "V", (items, k)), _dev(cache_v, torch.float64, "cache_v", (items, k))
+    _dev(Z, torch.float64, "Z", (z_rows, k)), _dev(cache_z, torch.float64, "cache_z", (z_rows, k))
     if loss is not None:
-        _dev(loss, torch.float64, "loss")
-        if loss.numel() != int(n_epochs) * n_total:
-            raise B200Error("loss must hold n_epochs * (n_edges + n_ratings) = %d values" % (int(n_epochs) * n_total))
+        _dev(loss, torch.float64, "loss", (int(n_epochs), data.n_edges + data.n_ratings))
     check(L.b200_cofactor_fit(COFACTOR_VARIANTS[data.variant], ptr(data.a_id), ptr(data.b_id), ptr(data.val),
-                              ptr(data.is_edge), ptr(data.level_ptr), data.n_levels, data.n_edges, data.n_ratings, k,
+                              ptr(data.is_edge), ptr(data.level_ptr), data.n_levels, data.n_edges, data.n_ratings, int(k),
                               ptr(U), ptr(V), ptr(Z), ptr(cache_u), ptr(cache_v), ptr(cache_z), int(n_epochs),
                               float(lambda_c), float(lambda_reg), float(learning_rate), float(gamma), ptr(loss),
                               ptr(data.order) if loss is not None else None, current_stream()), "b200_cofactor_fit")
@@ -995,31 +1029,20 @@ def nmf_fit(data, U, V, Bu, Bi, n_epochs, mu=0.0, learning_rate=0.005, lambda_u=
     V, Bu, Bi in place, bit for bit as the reference's serial loop.  The biases are trained when data.use_bias; they enter
     the predictions either way.  The hyperparameters are rounded to f32.  loss: optional f64 device tensor [n_epochs]
     that receives each epoch's sum err^2 + lambda_u |U|^2 + lambda_v |V|^2 (f64, not the reference's f32 order).
-    workspace: optional f32 device tensor shaped like U (allocated per call otherwise)."""
+    workspace: optional f32 device tensor of at least U.numel() floats, not U itself (allocated per call otherwise)."""
     L = require_cuda()
-    k = int(U.shape[1]) if U.dim() == 2 else 0
-    for t, name, rows in ((U, "U", data.n_users), (V, "V", data.n_items)):
-        _dev(t, torch.float32, name)
-        if t.dim() != 2 or int(t.shape[0]) != rows or int(t.shape[1]) != k or k < 1:
-            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, max(k, 1), tuple(t.shape)))
-    for t, name, rows in ((Bu, "Bu", data.n_users), (Bi, "Bi", data.n_items)):
-        _dev(t, torch.float32, name)
-        if t.numel() != rows:
-            raise B200Error("%s must hold %d values, got %d" % (name, rows, t.numel()))
+    k = _dev(U, torch.float32, "U", (data.n_users, _AtLeast(1))).shape[1]
+    _dev(V, torch.float32, "V", (data.n_items, k))
+    _dev(Bu, torch.float32, "Bu", data.n_users), _dev(Bi, torch.float32, "Bi", data.n_items)
     if loss is not None:
-        _dev(loss, torch.float64, "loss")
-        if loss.numel() != int(n_epochs):
-            raise B200Error("loss must hold n_epochs = %d values" % int(n_epochs))
-    if workspace is None:
-        workspace = torch.empty_like(U)
-    _dev(workspace, torch.float32, "workspace")
-    if workspace.numel() < U.numel() or workspace.data_ptr() == U.data_ptr():
-        raise B200Error("workspace must hold U.numel() floats and must not alias U")
-    f32 = lambda x: float(np.float32(x))              # noqa: E731
+        _dev(loss, torch.float64, "loss", int(n_epochs))
+    workspace = _buf(workspace, torch.float32, "workspace", _AtLeast(U.numel()))
+    if workspace.data_ptr() == U.data_ptr():
+        raise B200Error("workspace must not alias U")
     check(L.b200_nmf_fit(data.n_users, data.n_items, *data.ratings.args(), ptr(data.item_order), ptr(data.s_uid),
-                         ptr(data.s_iid), ptr(data.s_rat), ptr(data.s_pos), ptr(data.level_ptr), data.n_levels, k, ptr(U),
-                         ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs), f32(mu), f32(learning_rate),
-                         f32(lambda_u), f32(lambda_v), f32(lambda_bu), f32(lambda_bi), int(data.use_bias), ptr(loss),
+                         ptr(data.s_iid), ptr(data.s_rat), ptr(data.s_pos), ptr(data.level_ptr), data.n_levels, int(k), ptr(U),
+                         ptr(V), ptr(Bu), ptr(Bi), ptr(data.rp), ptr(workspace), int(n_epochs), _f32(mu), _f32(learning_rate),
+                         _f32(lambda_u), _f32(lambda_v), _f32(lambda_bu), _f32(lambda_bi), int(data.use_bias), ptr(loss),
                          current_stream()), "b200_nmf_fit")
 
 
@@ -1053,26 +1076,16 @@ def efm_fit(data, U1, U2, V, H1, H2, n_iter, lambda_x=1.0, lambda_y=1.0, lambda_
     loss, summed in f64 (not the reference's f32 order).  workspace: optional f32 device tensor of
     efm_workspace_floats(...) floats (allocated per call otherwise)."""
     L_ = require_cuda()
-    E = int(U1.shape[1]) if U1.dim() == 2 else 0
-    Lw = int(H1.shape[1]) if H1.dim() == 2 else 0
-    for t, name, shape in ((U1, "U1", (data.n_users, E)), (U2, "U2", (data.n_items, E)), (V, "V", (data.n_aspects, E)),
-                           (H1, "H1", (data.n_users, Lw)), (H2, "H2", (data.n_items, Lw))):
-        _dev(t, torch.float32, name)
-        if tuple(t.shape) != shape or E < 1 or Lw < 1:
-            raise B200Error("%s must have shape %s, got %s" % (name, shape, tuple(t.shape)))
+    E = _dev(U1, torch.float32, "U1", (data.n_users, _AtLeast(1))).shape[1]
+    Lw = _dev(H1, torch.float32, "H1", (data.n_users, _AtLeast(1))).shape[1]
+    _dev(U2, torch.float32, "U2", (data.n_items, E)), _dev(V, torch.float32, "V", (data.n_aspects, E))
+    _dev(H2, torch.float32, "H2", (data.n_items, Lw))
     if loss is not None:
-        _dev(loss, torch.float64, "loss")
-        if loss.numel() != int(n_iter):
-            raise B200Error("loss must hold n_iter = %d values" % int(n_iter))
+        _dev(loss, torch.float64, "loss", int(n_iter))
     need = efm_workspace_floats(data.n_users, data.n_items, data.n_aspects, E, Lw)
-    if workspace is None:
-        workspace = torch.empty(max(need, 1), dtype=torch.float32, device="cuda")
-    _dev(workspace, torch.float32, "workspace")
-    if workspace.numel() < need:
-        raise B200Error("workspace must hold %d floats" % need)
-    f32 = lambda x: float(np.float32(x))              # noqa: E731
-    check(L_.b200_efm_fit(*data.args(), E, Lw, ptr(U1), ptr(U2), ptr(V), ptr(H1), ptr(H2), ptr(workspace), ptr(data.pred),
-                          int(n_iter), f32(lambda_x), f32(lambda_y), f32(lambda_u), f32(lambda_h), f32(lambda_v),
+    workspace = _buf(workspace, torch.float32, "workspace", _AtLeast(need))
+    check(L_.b200_efm_fit(*data.args(), int(E), int(Lw), ptr(U1), ptr(U2), ptr(V), ptr(H1), ptr(H2), ptr(workspace), ptr(data.pred),
+                          int(n_iter), _f32(lambda_x), _f32(lambda_y), _f32(lambda_u), _f32(lambda_h), _f32(lambda_v),
                           ptr(loss), current_stream()), "b200_efm_fit")
 
 
@@ -1085,13 +1098,12 @@ def efm_queries(U1, H1, V, num_most_cared, alpha, rating_scale, user_idx=None):
     """[n_q, E + L] f32 query vectors of the aspect-weighted rank (b200_efm_queries) of the users user_idx (int64 device
     tensor; None: every row of U1): Q[q] . [U2 | H2][i] is EFM.rank's row alpha * explicit + (1 - alpha) * score."""
     L_ = require_cuda()
-    for t, name in ((U1, "U1"), (H1, "H1"), (V, "V")):
-        _dev(t, torch.float32, name)
-    E, Lw = int(U1.shape[1]), int(H1.shape[1])
-    if H1.shape[0] != U1.shape[0] or V.dim() != 2 or (V.shape[0] and int(V.shape[1]) != E):
-        raise B200Error("U1 %s, H1 %s and V %s do not agree in shape" % (tuple(U1.shape), tuple(H1.shape), tuple(V.shape)))
+    n_users, E = _dev(U1, torch.float32, "U1", (None, None)).shape
+    Lw = _dev(H1, torch.float32, "H1", (n_users, None)).shape[1]
+    if _dev(V, torch.float32, "V", (None, None)).shape[0]:           # without aspects V's width is never read
+        _dev(V, torch.float32, "V", (None, E))
     if user_idx is None:
-        user_idx = torch.arange(U1.shape[0], dtype=torch.int64, device=U1.device)
+        user_idx = torch.arange(n_users, dtype=torch.int64, device=U1.device)
     _dev(user_idx, torch.int64, "user_idx")
     Q = torch.empty((user_idx.numel(), E + Lw), dtype=torch.float32, device=U1.device)
     check(L_.b200_efm_queries(ptr(user_idx), user_idx.numel(), ptr(U1), ptr(H1), ptr(V), int(V.shape[0]), E, Lw,
@@ -1240,43 +1252,28 @@ def _tensor_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, n_pair, lr, lam
     L_ = require_cuda()
     comparer = isinstance(data, ComparerDeviceData)
     n_counts = 3 if comparer else 2
-    U, I, A, O, G1, G2, G3 = params
-    dims = (int(G1.shape[0]), int(G1.shape[1]), int(G2.shape[1]), int(G2.shape[2]))
-    d1, d2, d3, d4 = dims
+    G1, G2 = params[4:6]
+    d1, d2, d3 = _dev(G1, torch.float32, "G1", (None, None, None)).shape
+    d4 = _dev(G2, torch.float32, "G2", (d1, d3, None)).shape[2]
+    dims = (d1, d2, d3, d4)
     shapes = ((data.n_users, d1), (data.n_items, d2), (data.n_aspects + 1, d3), (data.n_opinions, d4), (d1, d2, d3),
               (d1, d3, d4), (d2, d3, d4))
     for name, t, st, shape in zip(MTER_PARAMS, params, sgrad, shapes):
-        _dev(t, torch.float32, name), _dev(st, torch.float32, "sgrad_" + name)
-        if tuple(t.shape) != shape or tuple(st.shape) != shape:
-            raise B200Error("%s and its AdaGrad sum must have shape %s, got %s / %s"
-                            % (name, shape, tuple(t.shape), tuple(st.shape)))
-    per_iter = 3 * int(n_el) + 2 * int(n_bpr) + int(n_pair)
+        _dev(t, torch.float32, name, shape), _dev(st, torch.float32, "sgrad_" + name, shape)
     if philox_seed is None:
-        _dev(draws, torch.int32, "draws")
-        if draws.numel() < int(n_iter) * per_iter:
-            raise B200Error("draws must hold n_iter * (3 n_el + 2 n_bpr%s) = %d values"
-                            % (" + n_pair" if comparer else "", int(n_iter) * per_iter))
+        _dev(draws, torch.int32, "draws", _AtLeast(int(n_iter) * (3 * int(n_el) + 2 * int(n_bpr) + int(n_pair))))
     else:
         draws = None
     if phase_ns is not None:
-        _dev(phase_ns, torch.int64, "phase_ns")
-    if counts is None:
-        counts = torch.zeros(n_counts, dtype=torch.int64, device="cuda")
-    _dev(counts, torch.int64, "counts")
+        _dev(phase_ns, torch.int64, "phase_ns", _AtLeast(4))
+    counts = _buf(counts, torch.int64, "counts", _AtLeast(n_counts), zero=True)
     if losses is not None:
-        _dev(losses, torch.float64, "losses")
-    if comparer and (counts.numel() < 3 or (losses is not None and losses.numel() < 3)):
-        raise B200Error("counts and losses must hold 3 values")
+        _dev(losses, torch.float64, "losses", _AtLeast(n_counts))
     need = (comparer_sub_workspace_bytes(data, dims, n_el, n_bpr, n_pair) if comparer else
             mter_workspace_bytes(data, dims, n_el, n_bpr))
-    if workspace is None:
-        workspace = torch.zeros(need, dtype=torch.uint8, device="cuda")
-    _dev(workspace, torch.uint8, "workspace")
-    if workspace.numel() < need:
-        raise B200Error("workspace must hold %d bytes" % need)
+    workspace = _buf(workspace, torch.uint8, "workspace", _AtLeast(need), zero=True)
     pp = (ctypes.c_void_p * 7)(*[ptr(t) for t in params])
     ps = (ctypes.c_void_p * 7)(*[ptr(t) for t in sgrad])
-    f32 = lambda x: float(np.float32(x))              # noqa: E731
     head = [*data.args(), *dims, *[ptr(t) for t in data.x], data.n_x, *[ptr(t) for t in data.yu], data.n_yu,
             *[ptr(t) for t in data.yi], data.n_yi, *[ptr(t) for t in data.csr], data.nnz]
     flags = (_lib.MTER_UNORDERED if unordered else 0) | (0 if philox_seed is None else _lib.MTER_PHILOX)
@@ -1284,12 +1281,12 @@ def _tensor_fit(data, params, sgrad, draws, n_iter, n_el, n_bpr, n_pair, lr, lam
             current_stream()]
     if comparer:
         check(L_.b200_comparer_sub_fit(*head, *[ptr(t) for t in data.pairs], data.n_plist, int(n_el), int(n_bpr),
-                                       int(n_pair), int(n_iter), ptr(draws), pp, ps, ptr(workspace), f32(lr),
-                                       f32(lambda_reg), f32(lambda_bpr), f32(lambda_d), *tail),
+                                       int(n_pair), int(n_iter), ptr(draws), pp, ps, ptr(workspace), _f32(lr),
+                                       _f32(lambda_reg), _f32(lambda_bpr), _f32(lambda_d), *tail),
               "b200_comparer_sub_fit")
     else:
-        check(L_.b200_mter_fit(*head, int(n_el), int(n_bpr), int(n_iter), ptr(draws), pp, ps, ptr(workspace), f32(lr),
-                               f32(lambda_reg), f32(lambda_bpr), *tail),
+        check(L_.b200_mter_fit(*head, int(n_el), int(n_bpr), int(n_iter), ptr(draws), pp, ps, ptr(workspace), _f32(lr),
+                               _f32(lambda_reg), _f32(lambda_bpr), *tail),
               "b200_mter_fit")
     return counts
 
@@ -1298,11 +1295,8 @@ def mter_queries(U, G1, A):
     """[n_users, d2] f32 rank queries (b200_mter_queries): Q[u] . I[i] is MTER.score(u)[i] = einsum(G1, U[u], I[i],
     A[-1]) up to rounding.  M = G1 . A[-1] and Q = U . M are f64 sums in index order, each rounded once to f32."""
     L_ = require_cuda()
-    for t, name in ((U, "U"), (G1, "G1"), (A, "A")):
-        _dev(t, torch.float32, name)
-    d1, d2, d3 = (int(x) for x in G1.shape)
-    if U.dim() != 2 or int(U.shape[1]) != d1 or A.dim() != 2 or int(A.shape[1]) != d3 or A.shape[0] < 1:
-        raise B200Error("U %s, G1 %s and A %s do not agree in shape" % (tuple(U.shape), tuple(G1.shape), tuple(A.shape)))
+    d1, d2, d3 = _dev(G1, torch.float32, "G1", (None, None, None)).shape
+    _dev(U, torch.float32, "U", (None, d1)), _dev(A, torch.float32, "A", (_AtLeast(1), d3))
     Q = torch.empty((U.shape[0], d2), dtype=torch.float32, device=U.device)
     check(L_.b200_mter_queries(ptr(U), int(U.shape[0]), ptr(G1), ptr(A[-1]), d1, d2, d3, ptr(Q), current_stream()),
           "b200_mter_queries")
@@ -1315,23 +1309,14 @@ def comparer_rank_rows(U, I, A, G1, user_idx, n_top, alpha, n_items=None, out=No
     + (1 - alpha) * ts3[i, n_aspects] with ts3[i, a] = sum_qr I[i, q] (sum_p G1[p, q, r] U[u, p]) A[a, r], every sum in
     f64 and one rounding to f32.  out: an optional [n_q, n_items] f32 device buffer to write."""
     L_ = require_cuda()
-    for t, name in ((U, "U"), (I, "I"), (A, "A"), (G1, "G1")):
-        _dev(t, torch.float32, name)
-    _dev(user_idx, torch.int64, "user_idx")
-    d1, d2, d3 = (int(x) for x in G1.shape)
-    if (U.dim() != 2 or int(U.shape[1]) != d1 or I.dim() != 2 or int(I.shape[1]) != d2 or A.dim() != 2
-            or int(A.shape[1]) != d3 or A.shape[0] < 2):
-        raise B200Error("U %s, I %s, A %s and G1 %s do not agree in shape"
-                        % (tuple(U.shape), tuple(I.shape), tuple(A.shape), tuple(G1.shape)))
-    n_items = int(I.shape[0]) if n_items is None else int(n_items)
-    if not 0 <= n_items <= int(I.shape[0]):
-        raise B200Error("n_items=%d outside [0, %d]" % (n_items, int(I.shape[0])))
-    n_q = user_idx.numel()
-    if out is None:
-        out = torch.empty((n_q, n_items), dtype=torch.float32, device=U.device)
-    elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()
-              and tuple(out.shape) == (n_q, n_items)):
-        raise B200Error("out must be a contiguous f32 CUDA tensor of shape %s" % ((n_q, n_items),))
+    d1, d2, d3 = _dev(G1, torch.float32, "G1", (None, None, None)).shape
+    _dev(U, torch.float32, "U", (None, d1)), _dev(A, torch.float32, "A", (_AtLeast(2), d3))
+    _dev(I, torch.float32, "I", (None if n_items is None else _AtLeast(n_items), d2))
+    n_items = int(I.shape[0] if n_items is None else n_items)
+    if n_items < 0:
+        raise B200Error("n_items must be >= 0, got %d" % n_items)
+    n_q = _dev(user_idx, torch.int64, "user_idx").numel()
+    out = _buf(out, torch.float32, "out", (n_q, n_items))
     check(L_.b200_comparer_rank_rows(ptr(U), ptr(I), ptr(A), ptr(G1), ptr(user_idx), n_q, n_items, d1, d2, d3,
                                      int(A.shape[0]) - 1, int(n_top), float(alpha), ptr(out), current_stream()),
           "b200_comparer_rank_rows")
@@ -1372,17 +1357,12 @@ class HpfData(SparseLayout):
 
 
 def _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr):
-    k = int(Gs.shape[1]) if Gs.dim() == 2 else 0
-    for t, name, rows in ((Gs, "Gs", data.n_users), (Gr, "Gr", data.n_users), (Ls, "Ls", data.n_items),
-                          (Lr, "Lr", data.n_items)):
-        _dev(t, torch.float64, name)
-        if t.dim() != 2 or int(t.shape[0]) != rows or int(t.shape[1]) != k or k < 1:
-            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, max(k, 1), tuple(t.shape)))
-    for t, name, rows in ((Kr, "Kr", data.n_users), (Tr, "Tr", data.n_items)):
-        _dev(t, torch.float64, name)
-        if t.numel() != rows:
-            raise B200Error("%s must hold %d values, got %d" % (name, rows, t.numel()))
-    return k
+    """k of an HPF state, checked: Gs, Gr [n_users, k], Ls, Lr [n_items, k], Kr [n_users], Tr [n_items]."""
+    k = _dev(Gs, torch.float64, "Gs", (data.n_users, _AtLeast(1))).shape[1]
+    _dev(Gr, torch.float64, "Gr", (data.n_users, k))
+    _dev(Ls, torch.float64, "Ls", (data.n_items, k)), _dev(Lr, torch.float64, "Lr", (data.n_items, k))
+    _dev(Kr, torch.float64, "Kr", data.n_users), _dev(Tr, torch.float64, "Tr", data.n_items)
+    return int(k)
 
 
 def hpf_fit(data, hierarchical, Gs, Gr, Ls, Lr, Kr, Tr, max_iter):
@@ -1402,10 +1382,7 @@ def hpf_update(data, hierarchical, Lt, Lb, Gs, Gr, Ls, Lr, Kr, Tr):
     """One iteration of the fit from given expectations Lt [n_users, k] and Lb [n_items, k] (f64 device tensors)."""
     L = require_cuda()
     k = _hpf_state(data, Gs, Gr, Ls, Lr, Kr, Tr)
-    for t, name, rows in ((Lt, "Lt", data.n_users), (Lb, "Lb", data.n_items)):
-        _dev(t, torch.float64, name)
-        if tuple(t.shape) != (rows, k):
-            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, k, tuple(t.shape)))
+    _dev(Lt, torch.float64, "Lt", (data.n_users, k)), _dev(Lb, torch.float64, "Lb", (data.n_items, k))
     check(L.b200_hpf_update(int(bool(hierarchical)), data.n_users, data.n_items, k, *data.args(), ptr(Lt), ptr(Lb),
                             ptr(Gs), ptr(Gr), ptr(Ls), ptr(Lr), ptr(Kr), ptr(Tr), ptr(data.workspace(k)), current_stream()),
           "b200_hpf_update")
@@ -1415,14 +1392,9 @@ def hpf_expect(shape, rate, out=None):
     """exp(digamma(shape) - log(rate)) element-wise on f64 device tensors, with HPF's stored-entry rules: a term whose
     argument is <= 0 is dropped, and an entry with both dropped is 0."""
     L = require_cuda()
-    _dev(shape, torch.float64, "shape"), _dev(rate, torch.float64, "rate")
-    if shape.shape != rate.shape:
-        raise B200Error("shape and rate differ in shape: %s, %s" % (tuple(shape.shape), tuple(rate.shape)))
-    if out is None:
-        out = torch.empty_like(shape)
-    _dev(out, torch.float64, "out")
-    if out.shape != shape.shape:
-        raise B200Error("out must have shape %s" % (tuple(shape.shape),))
+    dims = tuple(_dev(shape, torch.float64, "shape").shape)
+    _dev(rate, torch.float64, "rate", dims)
+    out = _buf(out, torch.float64, "out", dims)
     check(L.b200_hpf_expect(ptr(shape), ptr(rate), shape.numel(), ptr(out), current_stream()), "b200_hpf_expect")
     return out
 
@@ -1472,24 +1444,23 @@ def _c2pf_args(graph, variant, at, bt, state):
     if variant not in C2PF_VARIANTS:
         raise B200Error("variant must be one of %s, got %r" % (sorted(C2PF_VARIANTS), variant))
     r = graph.ratings
-    Gs = state[0]
-    _dev(Gs, torch.float64, "Gs")
-    k = int(Gs.shape[1]) if Gs.dim() == 2 else 0
-    absent = {"c2pf": (), "tc2pf": ("L2s", "L2r"), "rc2pf": ("Ls", "Lr")}[variant]
-    names = ("Gs", "Gr", "Ls", "Lr", "L2s", "L2r")
-    for t, name, rows in zip(state[:6], names, (r.n_users, r.n_users) + (r.n_items,) * 4):
-        if name in absent:
-            continue
-        _dev(t, torch.float64, name)
-        if t.dim() != 2 or int(t.shape[0]) != rows or int(t.shape[1]) != k or k < 1:
-            raise B200Error("%s must have shape (%d, %d), got %s" % (name, rows, max(k, 1), tuple(t.shape)))
-    for t, name, size in zip(state[6:], ("L3s", "L3r", "T3r"), (max(graph.n_edges, 1),) * 2 + (r.n_items,)):
-        _dev(t, torch.float64, name)
-        if t.numel() != size:
-            raise B200Error("%s must hold %d values, got %d" % (name, size, t.numel()))
-    ptrs = [None if name in absent else ptr(t) for t, name in zip(state[:6], names)] + [ptr(t) for t in state[6:]]
-    return k, [C2PF_VARIANTS[variant], r.n_users, r.n_items, k, *r.args(), graph.n_edges, ptr(graph.c_ptr),
-               ptr(graph.c_row), ptr(graph.c_col), ptr(graph.c_mir), ptr(graph.util), float(at), float(bt)] + ptrs
+    Gs, Gr, Ls, Lr, L2s, L2r, L3s, L3r, T3r = state
+    k = _dev(Gs, torch.float64, "Gs", (r.n_users, _AtLeast(1))).shape[1]
+    _dev(Gr, torch.float64, "Gr", (r.n_users, k))
+    if variant == "rc2pf":
+        Ls = Lr = None
+    else:
+        _dev(Ls, torch.float64, "Ls", (r.n_items, k)), _dev(Lr, torch.float64, "Lr", (r.n_items, k))
+    if variant == "tc2pf":
+        L2s = L2r = None
+    else:
+        _dev(L2s, torch.float64, "L2s", (r.n_items, k)), _dev(L2r, torch.float64, "L2r", (r.n_items, k))
+    n_edges = max(graph.n_edges, 1)
+    _dev(L3s, torch.float64, "L3s", n_edges), _dev(L3r, torch.float64, "L3r", n_edges)
+    _dev(T3r, torch.float64, "T3r", r.n_items)
+    return int(k), [C2PF_VARIANTS[variant], r.n_users, r.n_items, int(k), *r.args(), graph.n_edges, ptr(graph.c_ptr),
+                    ptr(graph.c_row), ptr(graph.c_col), ptr(graph.c_mir), ptr(graph.util), float(at), float(bt),
+                    *[ptr(t) for t in (Gs, Gr, Ls, Lr, L2s, L2r, L3s, L3r, T3r)]]
 
 
 def c2pf_fit(graph, variant, at, bt, state, n_iter):
@@ -1510,22 +1481,14 @@ def c2pf_update(graph, variant, at, bt, state, expectations, given=(None, None, 
     L = require_cuda()
     k, args = _c2pf_args(graph, variant, at, bt, state)
     r = graph.ratings
-    absent = {"c2pf": (), "tc2pf": (2,), "rc2pf": (1,)}[variant]
+    absent = {"c2pf": None, "tc2pf": 2, "rc2pf": 1}[variant]             # L2b / Lb, which the variant has not
     sizes = (r.n_users * k, r.n_items * k, r.n_items * k, max(graph.n_edges, 1), r.n_items * k)
-    for j, (t, size) in enumerate(zip(expectations, sizes)):
-        if j in absent:
-            continue
-        _dev(t, torch.float64, "expectation %d" % j)
-        if t.numel() != size:
-            raise B200Error("expectation %d must hold %d values, got %d" % (j, size, t.numel()))
-    for j, (t, size) in enumerate(zip(given, sizes)):
-        if t is not None:
-            _dev(t, torch.float64, "given expectation %d" % j)
-            if t.numel() != size:
-                raise B200Error("given expectation %d must hold %d values, got %d" % (j, size, t.numel()))
-    opt = lambda t: None if t is None else ptr(t)                     # noqa: E731
-    check(L.b200_c2pf_update(*args, *[None if j in absent else ptr(t) for j, t in enumerate(expectations)],
-                             *[opt(t) for t in given], ptr(graph.workspace(k)), current_stream()), "b200_c2pf_update")
+    exps = [None if j == absent else _dev(t, torch.float64, "expectation %d" % j, n)
+            for j, (t, n) in enumerate(zip(expectations, sizes))]
+    given = [None if t is None else _dev(t, torch.float64, "given expectation %d" % j, n)
+             for j, (t, n) in enumerate(zip(given, sizes))]
+    check(L.b200_c2pf_update(*args, *map(ptr, exps), *map(ptr, given), ptr(graph.workspace(k)), current_stream()),
+          "b200_c2pf_update")
 
 
 def rank_pack_items(V, item_base=None, n_items=None):
@@ -1533,9 +1496,10 @@ def rank_pack_items(V, item_base=None, n_items=None):
     base folded in + the scaling scalars, as a uint8 CUDA tensor to pass to rank_topk(packed_items=...).  Valid as long as
     V / item_base do not change.  Returns None for shapes the tensor-core pass does not take."""
     L = require_cuda()
-    _dev(V, torch.float32, "V")
-    n_items = V.shape[0] if n_items is None else int(n_items)
-    k = int(V.shape[1])
+    k = _dev(V, torch.float32, "V", (None if n_items is None else _AtLeast(n_items), None)).shape[1]
+    n_items = int(V.shape[0] if n_items is None else n_items)
+    if item_base is not None:
+        _dev(item_base, torch.float32, "item_base", _AtLeast(n_items))
     nbytes = int(L.b200_rank_items_bytes(n_items, k))
     if nbytes <= 0:
         return None
@@ -1550,21 +1514,17 @@ def rank_topk(U, V, topk, user_idx=None, item_base=None, user_off=None, excl_ind
     """Fused score + exclusion + top-k on device tensors (b200_rank_topk).  Returns (ids int32 [n_q, topk],
     scores f32 [n_q, topk]) CUDA tensors ordered by (score desc, item id asc); ids are -1 padded.
     packed_items: result of rank_pack_items(V, item_base, n_items) for the SAME V / item_base / n_items (skips the two
-    passes over V that every call otherwise makes)."""
+    passes over V that every call otherwise makes).  workspace: optional uint8 device scratch of at least
+    b200_rank_topk_workspace_bytes(n_q, n_items, k, topk) bytes (allocated per call otherwise)."""
     L = require_cuda()
-    _dev(U, torch.float32, "U"), _dev(V, torch.float32, "V")
-    n_items = V.shape[0] if n_items is None else int(n_items)
-    n_q = U.shape[0] if user_idx is None else user_idx.numel()
-    k = int(V.shape[1])
+    n_items, k, n_q = _score_args(U, V, user_idx, n_items, torch.float32, item_base, user_off)
+    _exclusions(excl_indptr, excl_indices, n_q)
+    if packed_items is not None:                                   # built by rank_pack_items for this n_items and k
+        _dev(packed_items, torch.uint8, "packed_items", int(L.b200_rank_items_bytes(n_items, k)))
+    nbytes = int(L.b200_rank_topk_workspace_bytes(n_q, n_items, k, int(topk)))
+    workspace = _buf(workspace, torch.uint8, "workspace", _AtLeast(max(nbytes, 16)))
     ids = torch.empty((n_q, topk), dtype=torch.int32, device=U.device)
     sc = torch.empty((n_q, topk), dtype=torch.float32, device=U.device)
-    nbytes = int(L.b200_rank_topk_workspace_bytes(n_q, n_items, k, int(topk)))
-    if workspace is None or workspace.numel() < nbytes:
-        workspace = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=U.device)
-    if packed_items is not None:
-        _dev(packed_items, torch.uint8, "packed_items")
-        if packed_items.numel() != int(L.b200_rank_items_bytes(n_items, k)):
-            raise B200Error("packed_items was built for another item count / factor width")
     check(L.b200_rank_topk_packed(ptr(U), ptr(user_idx), n_q, ptr(V), n_items, k, ptr(item_base), ptr(user_off),
                                   ptr(excl_indptr), ptr(excl_indices), int(topk), ptr(ids), ptr(sc), ptr(packed_items),
                                   ptr(workspace), workspace.numel(), current_stream()), "b200_rank_topk")
@@ -1597,11 +1557,11 @@ def topk_metrics(ids, pos_indptr, pos_indices, kinds, ks, user_idx=None, topk=No
     ids int32 [n_q, >=topk] CUDA; pos_* the test-positives CSR (int64 / int32 CUDA); kinds / ks python lists.
     Returns a float64 CUDA tensor [n_metrics, n_q]."""
     L = require_cuda()
-    _dev(ids, torch.int32, "ids"), _dev(pos_indptr, torch.int64, "pos_indptr"), _dev(pos_indices, torch.int32, "pos_indices")
-    n_q, stride = ids.shape
+    n_q, stride = _dev(ids, torch.int32, "ids", (None, None if topk is None else _AtLeast(topk))).shape
     topk = stride if topk is None else int(topk)
+    _dev(pos_indptr, torch.int64, "pos_indptr"), _dev(pos_indices, torch.int32, "pos_indices")
     if user_idx is not None:
-        _dev(user_idx, torch.int64, "user_idx")
+        _dev(user_idx, torch.int64, "user_idx", _AtLeast(n_q))
     mk = torch.tensor(list(kinds), dtype=torch.int32).to(ids.device)
     kk = torch.tensor(list(ks), dtype=torch.int32).to(ids.device)
     out = torch.empty((len(kinds), n_q), dtype=torch.float64, device=ids.device)
@@ -1616,33 +1576,39 @@ def rank_counts(scores, pos_indptr, pos_indices, user_idx=None, excl_indptr=None
     score row q.  Returns (less int64 [len(pos_indices)], pos_score f32 [len(pos_indices)], n_cand int64 [n_q],
     before_first int64 [n_q]); `less` / `pos_score` are filled only at the positions of the listed users' positives."""
     L = require_cuda()
-    _dev(scores, torch.float32, "scores"), _dev(pos_indptr, torch.int64, "pos_indptr"), _dev(pos_indices, torch.int32, "pos_indices")
-    n_q, n_items = scores.shape
-    dev = scores.device
-    if less is None:
-        less = torch.zeros(max(pos_indices.numel(), 1), dtype=torch.int64, device=dev)
-    if pos_score is None:
-        pos_score = torch.zeros(max(pos_indices.numel(), 1), dtype=torch.float32, device=dev)
-    n_cand = torch.zeros(max(n_q, 1), dtype=torch.int64, device=dev)
-    before = torch.zeros(max(n_q, 1), dtype=torch.int64, device=dev)
+    n_q, n_items = _dev(scores, torch.float32, "scores", (None, None)).shape
+    _dev(pos_indptr, torch.int64, "pos_indptr")
+    n_pos = _dev(pos_indices, torch.int32, "pos_indices").numel()
     if user_idx is not None:
-        _dev(user_idx, torch.int64, "user_idx")
-    if excl_indptr is not None:
-        _dev(excl_indptr, torch.int64, "excl_indptr"), _dev(excl_indices, torch.int32, "excl_indices")
+        _dev(user_idx, torch.int64, "user_idx", _AtLeast(n_q))
+    _exclusions(excl_indptr, excl_indices, n_q)
+    less = _buf(less, torch.int64, "less", _AtLeast(n_pos), zero=True)
+    pos_score = _buf(pos_score, torch.float32, "pos_score", _AtLeast(n_pos), zero=True)
+    n_cand = torch.zeros(max(n_q, 1), dtype=torch.int64, device=scores.device)
+    before = torch.zeros(max(n_q, 1), dtype=torch.int64, device=scores.device)
     check(L.b200_rank_counts(ptr(scores), n_q, n_items, ptr(excl_indptr), ptr(excl_indices), ptr(user_idx), ptr(pos_indptr),
                              ptr(pos_indices), ptr(less), ptr(pos_score), ptr(n_cand), ptr(before), current_stream()),
           "b200_rank_counts")
     return less, pos_score, n_cand[:n_q], before[:n_q]
 
 
+def _delta_args(x, snapshot, delta):
+    """The element count of a replica exchange step, checked: x, snapshot and delta f32 [>= n], n = x.numel()."""
+    n = _dev(x, torch.float32, "x").numel()
+    _dev(snapshot, torch.float32, "snapshot", _AtLeast(n)), _dev(delta, torch.float32, "delta", _AtLeast(n))
+    return n
+
+
 def delta_make(x, snapshot, delta):
     L = require_cuda()
-    check(L.b200_delta_make(ptr(x), ptr(snapshot), ptr(delta), x.numel(), current_stream()), "b200_delta_make")
+    n = _delta_args(x, snapshot, delta)
+    check(L.b200_delta_make(ptr(x), ptr(snapshot), ptr(delta), n, current_stream()), "b200_delta_make")
 
 
 def delta_apply(x, snapshot, delta):
     L = require_cuda()
-    check(L.b200_delta_apply(ptr(x), ptr(snapshot), ptr(delta), x.numel(), current_stream()), "b200_delta_apply")
+    n = _delta_args(x, snapshot, delta)
+    check(L.b200_delta_apply(ptr(x), ptr(snapshot), ptr(delta), n, current_stream()), "b200_delta_apply")
 
 
 def device_info():
