@@ -15,7 +15,8 @@ def _dev(a, dtype=None):
 
 
 @pytest.mark.parametrize("k,n_items,n_q", [(1, 5, 3), (2, 2, 1), (10, 1682, 9), (32, 257, 17), (64, 1000, 8),
-                                           (100, 4099, 5), (128, 2048, 33), (200, 300, 2)])
+                                           (100, 4099, 5), (128, 2048, 33), (200, 300, 2),
+                                           (16, 7, 600000)])        # 75,000 query groups: the grid's y loop wraps
 def test_score_batch_bit_exact(k, n_items, n_q):
     from cornac_b200 import engine
     rng = np.random.RandomState(k * 7 + n_items)
