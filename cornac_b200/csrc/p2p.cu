@@ -68,8 +68,11 @@ __device__ bool wait_all(const unsigned int* my_flags, int phase, int world, uns
 // `world` times too far and the epochs oscillate with growing amplitude from 4 ranks on (tools/sim_localsgd.py).  The mean over
 // the ranks that changed an element is a convex combination of their local results: stable at any world size, and equal to the
 // sum wherever one rank alone touched the element.
+// peers_aligned: every replica pointer is 16-byte aligned (the host checks them; a view at a storage offset is not), else
+// the whole slice takes the scalar loop.
 __global__ void __launch_bounds__(THREADS) item_exchange_kernel(const Peers P, int rank, int world, float* __restrict__ snap,
-                                                                int64_t n, int64_t lo, int64_t hi, unsigned int seq, int mean_touched)
+                                                                int64_t n, int64_t lo, int64_t hi, unsigned int seq, int mean_touched,
+                                                                int peers_aligned)
 {
     unsigned int* my_flags = P.flags[rank];
     __shared__ int ok_s;
@@ -86,7 +89,7 @@ __global__ void __launch_bounds__(THREADS) item_exchange_kernel(const Peers P, i
     if (ok_s) {
         // ---- owned slice [lo, hi): new = snap + sum_r (x_r - snap), stored into every replica and the snapshot
         const int64_t len = hi - lo;
-        const bool vec = ((lo & 3) == 0) && ((reinterpret_cast<uintptr_t>(snap) & 15) == 0);
+        const bool vec = peers_aligned && ((lo & 3) == 0) && ((reinterpret_cast<uintptr_t>(snap) & 15) == 0);
         const int64_t n4 = vec ? len / 4 : 0;
         const int64_t stride = (int64_t)gridDim.x * THREADS;
         for (int64_t i = (int64_t)blockIdx.x * THREADS + threadIdx.x; i < n4; i += stride) {
@@ -201,12 +204,14 @@ extern "C" int b200_item_exchange(int rank, int world, void* const* x_peers, voi
     B200_REQUIRE(world >= 1 && world <= p2p::MAX_WORLD && rank >= 0 && rank < world, "b200_item_exchange: rank %d / world %d", rank, world);
     B200_REQUIRE(x_peers && flag_peers && snapshot_slice && n >= 0 && seq != 0, "b200_item_exchange: bad argument");
     p2p::Peers P;
+    int peers_aligned = 1;
     for (int r = 0; r < p2p::MAX_WORLD; ++r) {
         P.x[r] = r < world ? static_cast<float*>(x_peers[r]) : nullptr;
         P.flags[r] = r < world ? static_cast<unsigned int*>(flag_peers[r]) : nullptr;
         B200_REQUIRE(r >= world || (P.x[r] && P.flags[r]), "b200_item_exchange: missing peer pointer %d", r);
+        if (r < world && (reinterpret_cast<uintptr_t>(P.x[r]) & 15) != 0) peers_aligned = 0;
     }
-    // slices are cut at multiples of 4 floats so that every slice keeps 16-byte alignment
+    // slices are cut at multiples of 4 floats so that every slice of an aligned replica keeps 16-byte alignment
     const int64_t per = ((n + world - 1) / world + 3) & ~(int64_t)3;
     int64_t lo = per * rank, hi = lo + per;
     if (lo > n) lo = n;
@@ -215,7 +220,8 @@ extern "C" int b200_item_exchange(int rank, int world, void* const* x_peers, voi
     const int64_t cap = (int64_t)sm_count() * 4;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    p2p::item_exchange_kernel<<<(unsigned)blocks, p2p::THREADS, 0, (cudaStream_t)stream>>>(P, rank, world, snapshot_slice, n, lo, hi, seq, mean_touched);
+    p2p::item_exchange_kernel<<<(unsigned)blocks, p2p::THREADS, 0, (cudaStream_t)stream>>>(P, rank, world, snapshot_slice, n, lo, hi, seq,
+                                                                                       mean_touched, peers_aligned);
     ::b200::count_launch();
     B200_CUDA(cudaGetLastError());
     return B200_OK;

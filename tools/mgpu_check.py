@@ -43,18 +43,24 @@ def mf_check(rank, world):
 
 def exchange_check(rank, world):
     """PeerItemExchange (one fused NVLink kernel) against ItemReplicaSync (delta kernels + NCCL all-reduce) on the same
-    local changes: every replica ends at start + sum of all ranks' changes; the p2p result is bit-equal on all ranks."""
+    local changes: every replica ends at start + the mean over the ranks that changed an element of their changes; the
+    p2p result is bit-equal on all ranks.  The changes are row-sparse, different rows per rank: row i is changed by
+    (i + it) % (world + 1) of the ranks, so every count from 0 to world occurs."""
     ok = True
-    for n, reps in ((1_000_003, 3), (128 * 50_000, 2), (7, 2)):
+    for n, reps, k in ((1_000_003, 3, 1), (128 * 50_000, 2, 128), (7, 2, 1)):
         g = torch.Generator(device="cuda").manual_seed(100 + n)          # same start on every rank
         start = torch.randn(n, generator=g, device="cuda")
         xa, xb = start.clone(), start.clone()
         pa = parallel.PeerItemExchange([xa])
         pb = parallel.ItemReplicaSync([xb])
         want = start.double().clone()
+        rows = torch.arange(n, device="cuda") // k
         for it in range(reps):
             gl = torch.Generator(device="cuda").manual_seed(7 * n + 31 * it)
             deltas = [torch.randn(n, generator=gl, device="cuda") * 0.01 * (r + 1) for r in range(world)]     # known on every rank
+            hits = (rows + it) % (world + 1)
+            for r, d in enumerate(deltas):
+                d[(r - rows) % world >= hits] = 0        # rank r changes the rows whose run of hits consecutive ranks covers r
             xa += deltas[rank]
             xb += deltas[rank]
             pa.exchange()
