@@ -100,6 +100,10 @@ SIGNATURES = {
     "b200_comparer_sub_fit": (_int, [_i64] * 4 + [_int] * 4 + ([_vp] * 4 + [_i64]) * 3 + [_vp] * 4 + [_i64] +
                               [_vp] * 4 + [_i64] + [_int] * 4 + [_vp] * 4 + [_f32] * 4 + [_int, _u64, _u64] + [_vp] * 4),
     "b200_comparer_rank_rows": (_int, [_vp] * 5 + [_i64, _i64] + [_int] * 3 + [_i64, _int, _c.c_double, _vp, _vp]),
+    "b200_lrppm_workspace_bytes": (_i64, [_i64] * 3 + [_int] * 3),
+    "b200_lrppm_fit": (_int, [_i64] * 3 + [_int] + [_vp] * 3 + [_i64] + [_vp] * 4 + [_i64] + [_vp, _i64, _vp, _vp, _i64] +
+                       [_int] * 3 + [_vp] * 3 + [_f32] * 3 + [_int, _u64, _u64] + [_vp] * 4),
+    "b200_lrppm_rank_rows": (_int, [_vp] * 8 + [_i64, _i64, _int, _i64, _int, _c.c_double, _c.c_double, _vp, _vp]),
     "b200_score": (_int, [_vp, _i64, _vp, _i64, _int, _vp, _f32, _vp, _vp]),
     "b200_score_batch": (_int, [_vp, _vp, _i64, _vp, _i64, _int, _vp, _vp, _vp, _vp]),
     "b200_topk_rows": (_int, [_vp, _i64, _i64, _vp, _vp, _int, _vp, _vp, _vp]),
@@ -134,6 +138,7 @@ BPR_DETERMINISTIC = 64
 PMF_LINEAR, PMF_NON_LINEAR = 0, 1
 COFACTOR_SOREC, COFACTOR_MCF = 0, 1
 MTER_UNORDERED, MTER_PHILOX = 1, 2
+LRPPM_PHILOX = 1
 SPD_POTRF, SPD_TRTRI, SPD_LAUUM, SPD_ALL = 1, 2, 4, 7
 METRIC_NDCG, METRIC_PRECISION, METRIC_RECALL, METRIC_FMEASURE, METRIC_HIT, METRIC_NCRR = range(6)
 

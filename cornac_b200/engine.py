@@ -18,6 +18,7 @@ functions mirror the reference kernels one to one (see include/b200cornac.h):
     efm_fit / efm_queries   <-> EFM._fit_efm / EFM.rank  (cornac/models/efm/recom_efm.pyx:268-353, 471-528)
     mter_fit / mter_queries <-> MTER._fit_mter / MTER.score (cornac/models/mter/recom_mter.pyx:434-714)
     comparer_sub_fit / comparer_rank_rows <-> ComparERSub._fit_mter / rank (recom_comparer_sub.pyx:487-806)
+    lrppm_fit / lrppm_rank_rows <-> LRPPM._fit / LRPPM.rank (cornac/models/lrppm/recom_lrppm.pyx:356-560)
 """
 import ctypes
 
@@ -1128,18 +1129,17 @@ class MterData:
         self.__dict__.update(kw)
 
 
-class MterDraws:
-    """The five seeded sample streams, drawn on the host in chunks of iterations and uploaded through two pinned
-    buffers: chunk k + 1 is drawn while the GPU runs chunk k.  `extra`: (seed, hi, n) of further streams, whose n draws
-    of an iteration follow the five's."""
+class StreamDraws:
+    """Seeded mt19937 sample streams (the reference's RNGVector, one thread each), drawn on the host in chunks of
+    iterations and uploaded through two pinned buffers: chunk k + 1 is drawn while the GPU runs chunk k.  streams:
+    (seed, hi, n) per stream, n draws in [0, hi] per iteration; an iteration's draws are the streams' in that order."""
 
-    def __init__(self, seeds, data, n_el, n_bpr, max_chunk, extra=()):
-        self.samplers = [MTSampler(s) for s in seeds] + [MTSampler(s) for s, _, _ in extra]
-        self.hi = [len(data.X) - 1, len(data.YU) - 1, len(data.YI) - 1, len(data.indices) - 1, data.n_items - 1]
-        self.hi += [int(hi) for _, hi, _ in extra]
-        self.n = [n_el, n_el, n_el, n_bpr, n_bpr] + [int(n) for _, _, n in extra]
+    def __init__(self, streams, max_chunk):
+        self.samplers = [MTSampler(int(s)) for s, _, _ in streams]
+        self.hi = [int(hi) for _, hi, _ in streams]
+        self.n = [int(n) for _, _, n in streams]
         self.per_iter = sum(self.n)
-        self.chunk = max(1, min(int(max_chunk), _MTER_DRAW_CHUNK // self.per_iter))
+        self.chunk = max(1, min(int(max_chunk), _MTER_DRAW_CHUNK // max(self.per_iter, 1)))
         self.host = [torch.empty((self.chunk, self.per_iter), dtype=torch.int32).pin_memory() for _ in range(2)]
         self.dev = [torch.empty((self.chunk, self.per_iter), dtype=torch.int32, device="cuda") for _ in range(2)]
         self.done = [None, None]
@@ -1163,6 +1163,16 @@ class MterDraws:
         self.done[k] = torch.cuda.Event()
         self.done[k].record()
         return dev
+
+
+class MterDraws(StreamDraws):
+    """MTER's five seeded sample streams (uia, uao, iao, pos, neg) as StreamDraws.  `extra`: (seed, hi, n) of further
+    streams, whose n draws of an iteration follow the five's."""
+
+    def __init__(self, seeds, data, n_el, n_bpr, max_chunk, extra=()):
+        his = [len(data.X) - 1, len(data.YU) - 1, len(data.YI) - 1, len(data.indices) - 1, data.n_items - 1]
+        ns = [n_el, n_el, n_el, n_bpr, n_bpr]
+        super().__init__(list(zip(seeds, his, ns)) + list(extra), max_chunk)
 
 
 class MterDeviceData:
@@ -1320,6 +1330,123 @@ def comparer_rank_rows(U, I, A, G1, user_idx, n_top, alpha, n_items=None, out=No
     check(L_.b200_comparer_rank_rows(ptr(U), ptr(I), ptr(A), ptr(G1), ptr(user_idx), n_q, n_items, d1, d2, d3,
                                      int(A.shape[0]) - 1, int(n_top), float(alpha), ptr(out), current_stream()),
           "b200_comparer_rank_rows")
+    return out
+
+
+LRPPM_PARAMS = ("U", "I", "UA", "IA")
+
+
+class LrppmData:
+    """The arrays LRPPM.fit hands to `_fit` (recom_lrppm.pyx:289-303) and the lookups its loop makes, in the reference's
+    order.  u_indices / i_indices / r_values: the train set's triples; X_uids / X_iids / X_aids / X_l_ui: the review
+    triples and their weights; aspect_keys: the sorted distinct wrapped get_key3 keys of the triples; rating_keys /
+    rating_values: the sorted distinct wrapped get_key(u, i) keys of the ratings with the f32 value the reference's
+    IntFloatDict keeps; item_aspect_quality: the f64 item x aspect quality CSR."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+class LrppmDeviceData:
+    """Device copy of an LrppmData, uploaded once per fit."""
+
+    def __init__(self, data):
+        i32 = lambda a: to_device(_pad(np.asarray(a, dtype=np.int32)), torch.int32)      # noqa: E731
+        f32 = lambda a: to_device(_pad(np.asarray(a, dtype=np.float32)), torch.float32)  # noqa: E731
+        self.n_users, self.n_items, self.n_aspects = int(data.n_users), int(data.n_items), int(data.n_aspects)
+        self.ratings = [i32(data.u_indices), i32(data.i_indices), f32(data.r_values)]
+        self.n_r = len(data.r_values)
+        self.triples = [i32(data.X_uids), i32(data.X_iids), i32(data.X_aids), f32(data.X_l_ui)]
+        self.n_x = len(data.X_uids)
+        self.akeys = i32(data.aspect_keys)
+        self.n_akeys = len(data.aspect_keys)
+        self.rkeys, self.rvals = i32(data.rating_keys), f32(data.rating_values)
+        self.n_rkeys = len(data.rating_keys)
+
+
+def lrppm_draws(seeds, data, n_samples, n_ranking_samples, max_chunk):
+    """LRPPM's three seeded streams (pos, pos_uia, neg_uia; recom_lrppm.pyx:307-309) as StreamDraws."""
+    pos, pos_uia, neg_uia = seeds
+    return StreamDraws([(pos, len(data.r_values) - 1, n_samples), (pos_uia, len(data.X_uids) - 1, n_ranking_samples),
+                        (neg_uia, data.n_aspects - 1, n_ranking_samples)], max_chunk)
+
+
+def lrppm_workspace_bytes(data, k, n_samples, n_ranking_samples):
+    L_ = require_cuda()
+    return int(L_.b200_lrppm_workspace_bytes(data.n_users, data.n_items, data.n_aspects, int(k), int(n_samples),
+                                             int(n_ranking_samples)))
+
+
+def lrppm_fit(data, params, draws, n_iter, n_samples, n_ranking_samples, lr=0.1, reg=0.01, ld=1.0, counts=None,
+              losses=None, workspace=None, philox_seed=None, iter0=0, phase_ns=None):
+    """Up to n_iter iterations of LRPPM._fit (recom_lrppm.pyx:356-482) over `data` (LrppmDeviceData), bit for bit as the
+    reference's compiled float loop given the draws; the fit stops after the first iteration that leaves every
+    parameter isclose to its value before it (recom_lrppm.pyx:337-344).  params: the f32 device tensors U, I, UA, IA,
+    updated in place.  draws: int32 device tensor [n_iter, n_samples + 2 n_ranking_samples] (pos, pos_uia, neg_uia).
+    counts: int64 device [4] (+= correct, skipped, iterations run; [3] = 1 once converged).  losses: f64 device [3] or
+    None (+= loss, ranking_loss, r_loss).  workspace: uint8 device tensor of lrppm_workspace_bytes that is zero before
+    its first use.  philox_seed: draw on the device from Philox4x32-10 with this key, iterations iter0, iter0 + 1, ...
+    (draws is then ignored).  phase_ns: int64 device [3] or None (+= nanoseconds of the predictions, del chains, dense
+    step)."""
+    L_ = require_cuda()
+    k = _dev(params[0], torch.float32, "U", (data.n_users, None)).shape[1]
+    for name, t, rows in zip(LRPPM_PARAMS, params, (data.n_users, data.n_items, data.n_aspects, data.n_aspects)):
+        _dev(t, torch.float32, name, (rows, k))
+    n_s, n_rk = int(n_samples), int(n_ranking_samples)
+    if n_s < 0 or n_rk < 0:
+        raise B200Error("n_samples and n_ranking_samples must not be negative")
+    if philox_seed is None:
+        _dev(draws, torch.int32, "draws", _AtLeast(int(n_iter) * (n_s + 2 * n_rk)))
+    else:
+        draws = None
+    if phase_ns is not None:
+        _dev(phase_ns, torch.int64, "phase_ns", _AtLeast(3))
+    counts = _buf(counts, torch.int64, "counts", _AtLeast(4), zero=True)
+    if losses is not None:
+        _dev(losses, torch.float64, "losses", _AtLeast(3))
+    workspace = _buf(workspace, torch.uint8, "workspace", _AtLeast(lrppm_workspace_bytes(data, k, n_s, n_rk)), zero=True)
+    pp = (ctypes.c_void_p * 4)(*[ptr(t) for t in params])
+    check(L_.b200_lrppm_fit(data.n_users, data.n_items, data.n_aspects, int(k), *[ptr(t) for t in data.ratings],
+                            data.n_r, *[ptr(t) for t in data.triples], data.n_x, ptr(data.akeys), data.n_akeys,
+                            ptr(data.rkeys), ptr(data.rvals), data.n_rkeys, n_s, n_rk, int(n_iter), ptr(draws), pp,
+                            ptr(workspace), _f32(lr), _f32(reg), _f32(ld), 0 if philox_seed is None else _lib.LRPPM_PHILOX,
+                            int(philox_seed or 0) & (2 ** 64 - 1), int(iter0), ptr(counts), ptr(losses), ptr(phase_ns),
+                            current_stream()),
+          "b200_lrppm_fit")
+    return counts
+
+
+class LrppmQuality:
+    """Device copy of the f64 item x aspect quality CSR of a trained LRPPM."""
+
+    def __init__(self, Q):
+        Q = _sp.csr_matrix(Q)
+        self.n_rows, self.n_aspects = Q.shape
+        self.indptr = to_device(Q.indptr.astype(np.int32), torch.int32)
+        self.indices = to_device(_pad(Q.indices.astype(np.int32)), torch.int32)
+        self.data = to_device(_pad(Q.data.astype(np.float64)), torch.float64)
+
+
+def lrppm_rank_rows(U, I, UA, IA, quality, user_idx, n_top, alpha, rating_scale, n_items=None, out=None):
+    """[n_q, n_items] f64 device rank rows of LRPPM (b200_lrppm_rank_rows): for each user u of user_idx (int64 device)
+    and item i < n_items (default all rows of I), alpha rating_scale mean(the n_top largest s[i, a], each times
+    q[i, a]) + f32(f32(1 - alpha) f32(I[i] . U[u])), with s[i, a] = f32(f32(f32(UA[a] . U[u]) + f32(I[i] . IA[a])) +
+    f32(I[i] . U[u])).  quality: an LrppmQuality.  out: an optional [n_q, n_items] f64 device buffer to write."""
+    L_ = require_cuda()
+    k = _dev(U, torch.float32, "U", (None, None)).shape[1]
+    n_aspects = _dev(UA, torch.float32, "UA", (None, k)).shape[0]
+    _dev(IA, torch.float32, "IA", (n_aspects, k))
+    _dev(I, torch.float32, "I", (None if n_items is None else _AtLeast(n_items), k))
+    n_items = int(I.shape[0] if n_items is None else n_items)
+    if n_items < 0 or n_items > quality.n_rows or quality.n_aspects != n_aspects:
+        raise B200Error("quality of shape (%d, %d) for %d items and %d aspects" % (quality.n_rows, quality.n_aspects,
+                                                                                 n_items, n_aspects))
+    n_q = _dev(user_idx, torch.int64, "user_idx").numel()
+    out = _buf(out, torch.float64, "out", (n_q, n_items))
+    check(L_.b200_lrppm_rank_rows(ptr(U), ptr(I), ptr(UA), ptr(IA), ptr(quality.indptr), ptr(quality.indices),
+                                  ptr(quality.data), ptr(user_idx), n_q, n_items, int(k), int(n_aspects), int(n_top),
+                                  float(alpha), float(rating_scale), ptr(out), current_stream()),
+          "b200_lrppm_rank_rows")
     return out
 
 

@@ -713,6 +713,53 @@ B200_API int b200_comparer_rank_rows(const float* U, const float* I, const float
                                      int64_t n_aspects, int n_top, double alpha, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * LRPPM (cornac/models/lrppm/recom_lrppm.pyx:356-560): the fit, bit-identical to the reference's compiled float loop
+ * given the same draws, and its aspect-mixed rank rows.  Shapes: U [n_users, k], I [n_items, k], UA and IA
+ * [n_aspects, k], row-major device f32.
+ *
+ * b200_lrppm_fit: up to n_iter iterations in one cooperative launch.  It stops after the first iteration in which every
+ *   element of U, I, UA and IA is numpy-isclose (rtol 1e-5, atol 1e-8, in f32) to its value before that iteration, as
+ *   the reference's convergence test does.  Two calls of a and b iterations equal one call of a + b unless the first
+ *   call stops early.
+ *   r_u, r_i, r_val   int32 / f32 [n_r]: the train set's (user, item, rating) triples (the `pos` stream draws them)
+ *   x_u, x_i, x_a     int32 [n_x]: the review triples (user, item, aspect) in the reference's order, x_l f32 [n_x] their
+ *                     weight 1 / (cnt (n_aspects - cnt))
+ *   akeys             int32 [n_akeys]: sorted distinct get_key3(u, i, a) of the triples, in C int with two's-complement
+ *                     wrap (the skip test: a ranking sample is skipped when get_key3(u, i, a_j) is among them)
+ *   rkeys, rvals      int32 / f32 [n_rkeys]: sorted distinct get_key(u, i) of the ratings and the value the reference's
+ *                     IntFloatDict keeps for each (the last); an absent key reads 0
+ *   draws             int32 [n_iter][n_samples + 2 n_ranking_samples]: per iteration the pos, pos_uia and neg_uia
+ *                     draws; unused (may be NULL) with B200_LRPPM_PHILOX, which draws Philox4x32-10 of
+ *                     (draw, iter0 + it) with key `seed` on the device under the same uniform law
+ *   params            host array of 4 device pointers U, I, UA, IA, updated in place
+ *   work              device, b200_lrppm_workspace_bytes(...) bytes, zero before the first call; the fit leaves it so
+ *   lr, reg, ld       f32, as the reference's `floating` locals
+ *   counts            device u64[4]: += correct, skipped, iterations run; counts[3] = 1 when the fit converged
+ *   losses            device f64[3] or NULL: += loss, ranking_loss, r_loss, summed in f64 in no fixed order
+ *   phase_ns          device u64[3] or NULL: += the nanoseconds of the phases (predictions, del chains, dense step)
+ *
+ * b200_lrppm_rank_rows: out [n_q, n_items] f64, the rank rows of users[0..n_q) over items [0, n_items):
+ *   s[i, a] = f32(f32(f32(UA[a] . U[u]) + f32(I[i] . IA[a])) + f32(I[i] . U[u])), each dot an f64 index-order sum,
+ *   out[i] = alpha rating_scale (sum over the n_top largest s[i, :] of s q[i, a]) / n_top
+ *            + f32(f32(1 - alpha) f32(I[i] . U[u]))
+ *   q: the item x aspect quality CSR (f64, sorted or not; an absent entry is 0).  At a tie at the n_top-th place the
+ *   smaller aspect ids are taken.  0 < n_top <= n_aspects <= 1024.                                                    */
+#define B200_LRPPM_PHILOX 1
+B200_API int64_t b200_lrppm_workspace_bytes(int64_t n_users, int64_t n_items, int64_t n_aspects, int k, int n_samples,
+                                            int n_ranking_samples);
+B200_API int b200_lrppm_fit(int64_t n_users, int64_t n_items, int64_t n_aspects, int k, const int32_t* r_u,
+                            const int32_t* r_i, const float* r_val, int64_t n_r, const int32_t* x_u, const int32_t* x_i,
+                            const int32_t* x_a, const float* x_l, int64_t n_x, const int32_t* akeys, int64_t n_akeys,
+                            const int32_t* rkeys, const float* rvals, int64_t n_rkeys, int n_samples,
+                            int n_ranking_samples, int n_iter, const int32_t* draws, float* const* params, void* work,
+                            float lr, float reg, float ld, int flags, uint64_t seed, uint64_t iter0,
+                            unsigned long long* counts, double* losses, unsigned long long* phase_ns, void* stream);
+B200_API int b200_lrppm_rank_rows(const float* U, const float* I, const float* UA, const float* IA,
+                                  const int32_t* q_indptr, const int32_t* q_indices, const double* q_data,
+                                  const int64_t* users, int64_t n_q, int64_t n_items, int k, int64_t n_aspects,
+                                  int n_top, double alpha, double rating_scale, double* out, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Multi-GPU item-factor exchange (no reference counterpart: the reference is a single
  * process).  Each rank trains its user shard against a replica of V / B; at the epoch
  * boundary   b200_delta_make:  delta[i] = x[i] - snapshot[i]
